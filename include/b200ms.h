@@ -1,5 +1,5 @@
 /*
- * b200ms.h -- C ABI of the B200-native waveguide mode solver (libb200ms.so).
+ * b200ms.h -- C ABI of the H100-native waveguide mode solver (libb200ms.so).
  *
  * Drop-in boundary for the hot path of flexcompute/tidy3d's local mode solver.  Every entry point
  * names the reference interface it replaces (paths relative to the tidy3d tree):
@@ -179,7 +179,7 @@ typedef struct {
   int mg_nu;             /* Jacobi pre/post sweeps (default 2) */
   int mg_min_size;       /* stop coarsening below this many cells per axis (default 12) */
   int mg_coarse_iters;   /* Krylov iterations on the coarsest level (default 16) */
-  int max_batch;         /* problems solved concurrently on the device (default 64: 5120 CTAs of the fp64 apply = 4.94 waves on 148 SMs) */
+  int max_batch;         /* problems solved concurrently on the device (default 64) */
   double mg_omega;       /* Jacobi damping (default 0.8) */
   double mg_ppw;         /* indefinite problems: keep >= this many cells per local wavelength (default 4) */
   int verbose;

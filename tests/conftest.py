@@ -9,7 +9,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (H100)")
     config.addinivalue_line("markers", "reference: needs the reference tree under /root/reference (build container only)")
 
 

@@ -49,7 +49,7 @@ def _check_against_golden(name, fields, n, spec, preset):
     if "fields_tight" in g.files:
         ok = well_separated(g["n_tight"])
         ov = mode_overlaps(fields, g["fields_tight"])  # E and H blocks separately + their relative phase
-        # |eps| = 1e8 inside metal amplifies the eigenvector error at the reference's own (loose) tolerance: measured 0.9962
+        # |eps| = 1e8 inside metal amplifies the eigenvector error at the reference's own (loose) tolerance
         ov_min = 0.99 if ("pec" in name and preset == "reference") else OVERLAP_MIN
         assert (ov[ok] > ov_min).all(), ov
     # per-mode component amplitudes |E_x|..|H_z| (phase independent; catches a wrong H scale or a dropped component);

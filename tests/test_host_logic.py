@@ -333,7 +333,7 @@ def test_pair_kernel_strip_geometry_covers_every_column_pair_once(built_lib):
     L = built_lib.lib()
     W, S, R = C.c_int(), C.c_int(), C.c_int()
     for ny in list(range(8, 700, 2)) + [1024, 1100, 2048, 4096, 5000]:
-        assert L.b200ms_debug_march2_geometry(512, ny, 64, 296, C.byref(W), C.byref(S), C.byref(R)) == 0
+        assert L.b200ms_debug_march2_geometry(512, ny, 64, 264, C.byref(W), C.byref(S), C.byref(R)) == 0
         w, s, npairs = W.value, S.value, ny // 2
         assert w % 32 == 0 and 32 <= w <= 256
         owners = [0] * npairs
@@ -345,13 +345,14 @@ def test_pair_kernel_strip_geometry_covers_every_column_pair_once(built_lib):
         assert owners == [1] * npairs, (ny, w, s)
         if npairs <= w:
             assert s == 1
-    for nx, nb, res in ((512, 64, 296), (512, 32, 296), (256, 64, 592), (128, 64, 1184), (40, 1, 296), (33, 7, 148)):
+    for nx, nb, res in ((512, 64, 264), (512, 32, 264), (256, 64, 528), (128, 64, 1056), (40, 1, 264), (33, 7, 132)):
         assert L.b200ms_debug_march2_geometry(nx, 512, nb, res, C.byref(W), C.byref(S), C.byref(R)) == 0
         assert (R.value + 3) % 6 == 0 and 9 <= R.value <= 69
-    # the headline level: 64 problems of 512 x 512 on 296 resident CTAs -> 9 CTAs of 57 rows per problem = 576 CTAs, two full waves
-    assert L.b200ms_debug_march2_geometry(512, 512, 64, 296, C.byref(W), C.byref(S), C.byref(R)) == 0
-    assert (W.value, S.value, R.value) == (256, 1, 57)
-    assert L.b200ms_debug_march2_geometry(512, 511, 64, 296, C.byref(W), C.byref(S), C.byref(R)) != 0  # odd widths use the one-column kernel
+    # the headline level: 64 problems of 512 x 512 on 264 resident CTAs (H100: 132 SMs x 2) -> 8 CTAs of 69 rows per problem
+    # = 512 CTAs, two nearly full waves
+    assert L.b200ms_debug_march2_geometry(512, 512, 64, 264, C.byref(W), C.byref(S), C.byref(R)) == 0
+    assert (W.value, S.value, R.value) == (256, 1, 69)
+    assert L.b200ms_debug_march2_geometry(512, 511, 64, 264, C.byref(W), C.byref(S), C.byref(R)) != 0  # odd widths use the one-column kernel
 
 
 def test_host_setup_matches_oracle_on_random_specs(built_lib):

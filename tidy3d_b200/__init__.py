@@ -1,4 +1,4 @@
-"""tidy3d_b200 -- B200-native drop-in for the hot path of tidy3d's local mode solver.
+"""tidy3d_b200 -- H100-native drop-in for the hot path of tidy3d's local mode solver.
 
 Public surface (mirrors ``tidy3d.plugins.mode.solver``):
     compute_modes(eps_cross, coords, freq, mode_spec, ...) -> (fields, n_complex, eps_spec)

@@ -1,7 +1,6 @@
 // Fused multigrid tail: the V-cycle on all levels from `l0` down to the coarsest one in ONE kernel, one CTA per problem,
 // with the level vectors held in shared memory.  On those levels (<= 32^2 .. 64^2 cells) the separate kernels of the
-// unfused cycle are pure launch / dependency latency: ~45 launches of 3-27 us each per V-cycle whatever the batch size
-// (profiles/r02_launch_shares.txt); fused they are a few dozen block-synchronised passes over a few thousand cells.
+// unfused cycle are pure launch / dependency latency: ~45 short launches per V-cycle whatever the batch size; fused they are a few dozen block-synchronised passes over a few thousand cells.
 // The arithmetic is that of BatchSolver::vcycle (jacobi0, nu-1 pre-sweeps, residual, restriction, recursion, prolongation,
 // nu post-sweeps; n_sw Jacobi sweeps on the coarsest level) with the stored omega/diag smoother.
 #pragma once

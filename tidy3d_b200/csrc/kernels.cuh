@@ -1,4 +1,4 @@
-// Device kernels of the B200 mode solver (sm_100a).  All kernels are batched: blockIdx.z (or .y for
+// Device kernels of the mode solver (sm_90a).  All kernels are batched: blockIdx.z (or .y for
 // the 1-D kernels) is the problem index inside a batch of same-shaped eigenproblems.
 //
 // Vector layout: a "batched vector" is [B][2][nx][ny] (Ex then Ey, y fastest), scalar type T (double
@@ -69,7 +69,7 @@ HD void convert(cplxf s, cplx &d) { d = mk(s.re, s.im); }
 HD void convert(cplxf s, cplxf &d) { d = s; }
 
 // real scalar type matching a vector element type (transfer weights are converted to it once per thread: with double
-// weights the fp32 transfer kernels were instruction-bound on F2F conversions and DFMAs, profiles/r02_restrict_ncu.txt)
+// weights the fp32 transfer kernels were instruction-bound on F2F conversions and DFMAs)
 template <typename T> struct RealOf { using type = double; };
 template <> struct RealOf<float> { using type = float; };
 template <> struct RealOf<cplxf> { using type = float; };
@@ -341,9 +341,9 @@ __global__ void __launch_bounds__(256) stencil_kernel(StencilArgs<T, C> a) {
 // ------------------------------------------------------------------------------------------------
 constexpr int kMarchCols = 128, kMarchOut = 126;
 
-// Measured alternatives (bench.py --stencil-only, 32 x 512^2): a two-deep software prefetch (89 registers) ran the fp64
-// apply at 126 us and forcing 8 CTAs/SM through __launch_bounds__ (64 registers, small spills) at 131 us, against
-// 108 us for this one-deep version at 72 registers; occupancy and register pressure trade off right here.
+// Alternatives tried (bench.py --stencil-only): a two-deep software prefetch and forcing 8 CTAs/SM through __launch_bounds__
+// (64 registers, small spills) both ran the fp64 apply slower than this one-deep version; occupancy and register pressure
+// trade off right here.
 template <typename T, typename C, int MODE, bool HAS_MU, int TXR>
 __global__ void __launch_bounds__(kMarchCols) stencil_march_kernel(StencilArgs<T, C> a) {
   constexpr bool JAC = (MODE == MODE_JACOBI);
@@ -508,8 +508,8 @@ __global__ void __launch_bounds__(kMarchCols) stencil_march_kernel(StencilArgs<T
 // ------------------------------------------------------------------------------------------------
 // cp.async variant of the marching kernel (LDGSTS: asynchronous global -> shared copies, no staging registers).
 // Same march, same exchange of u / t through shared memory; what changes is how a thread gets its own column's row data:
-// instead of loading row k+3 into registers one step ahead (one global round trip per row step, the long-scoreboard stall
-// ncu shows for the register version), every thread keeps its next rows in flight as 4/8-byte cp.async copies into a
+// instead of loading row k+3 into registers one step ahead (one global round trip per row step, a long-scoreboard stall
+// in the register version), every thread keeps its next rows in flight as 4/8-byte cp.async copies into a
 // private four-slot ring in shared memory -- raw fields three row steps ahead, rhs / omega-over-diagonal one step ahead of
 // their use -- and waits with cp.async.wait_group.  No mu fields, no recomputed-diagonal mode (the multigrid hot path:
 // stored-diagonal sweep, residual, apply).
@@ -775,9 +775,9 @@ __global__ void __launch_bounds__(256) restrict_kernel(TransferArgs a, const T *
   coarse[((size_t)b * 2 + comp) * Nc + (size_t)I * a.nyc + J] = acc;
 }
 
-// Restriction from packed lists (fp32 multigrid).  ncu on restrict_kernel at 64 x 512^2 (profiles/r02_transfers_ncu.txt): 370
-// thread instructions per coarse value, issue slots 71 % busy, DRAM at 1.2 TB/s -- the loads of the four list ranges, sixteen
-// double -> float weight conversions and the per-term predicates, not the sixteen gathers, set the pace.  Here a coarse index'
+// Restriction from packed lists (fp32 multigrid).  restrict_kernel is instruction-issue-bound, not HBM-bound: the loads of
+// the four list ranges, sixteen double -> float weight conversions and the per-term predicates, not the sixteen gathers, set
+// the pace.  Here a coarse index'
 // list is one 32-byte record (two 128-bit loads), the weights are fp32, unused entries carry weight zero and a valid index, and the
 // sixteen gathers are unconditional.  Same summation order as restrict_kernel, so the results are identical.
 template <typename T>
@@ -815,8 +815,7 @@ __global__ void __launch_bounds__(256) restrict4_kernel(TransferArgs a, const T 
 // Shared-memory tiled restriction (element types of <= 8 bytes): a CTA produces an 8 x 64 tile of coarse values of one
 // component of one problem.  The fine window the tile depends on (<= 28 x 200 values for aggregates of <= 3 cells) is loaded
 // once with coalesced row reads; every coarse value is then a <= 4 x 4 weighted sum out of shared memory.  The per-thread
-// version above reads every fine value up to four times through L1 with stride-2 addresses and was the second largest
-// kernel of a V-cycle (162 us at 64 x 512^2 for 134 MB of input, profiles/r02_launch_shares.txt).
+// version above reads every fine value up to four times through L1 with stride-2 addresses.
 constexpr int kRtI = 8, kRtJ = 64, kRtRows = 28, kRtCols = 200;
 template <typename T>
 __global__ void __launch_bounds__(256) restrict_tiled_kernel(TransferArgs a, const T *fine, T *coarse) {

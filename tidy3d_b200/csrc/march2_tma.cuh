@@ -1,4 +1,4 @@
-// Pair-marching stencil with TMA row staging (cp.async.bulk + mbarrier), sm_100a.
+// Pair-marching stencil with TMA row staging (cp.async.bulk + mbarrier), sm_90a.
 //
 // Same march and the same arithmetic as stencil_march2_kernel (csrc/march2.cuh); what changes is how a row reaches the thread
 // that owns it.  A strip's slice of a grid row is contiguous in HBM (W column pairs = 8 W bytes per array), so one elected
@@ -7,7 +7,7 @@
 // memory, and every stage completes on its own mbarrier (expect_tx = the bytes of that step).  Rows in flight cost no registers
 // and no per-thread load instructions: with D = 3 two to three rows (18 KB each at W = 256) are in flight per CTA, against one
 // row of prefetch registers in the register version, which is what the register version's bandwidth is limited by
-// (Little's law: ~40 KB in flight per SM at 7.7 TB/s).  A stage is refilled by the elected thread right after the
+// (Little's law: bytes in flight per SM = HBM bandwidth x latency / SMs).  A stage is refilled by the elected thread right after the
 // __syncthreads that ends the step which consumed it (the march needs that barrier anyway), so no "empty" barriers exist.
 // Requirements beyond the register version: ny % 4 == 0 (16-byte aligned row slices).  MODE_JACOBI_D0 stays with the register
 // version.  A wait that does not complete within ~2^24 polls traps instead of hanging the device.

@@ -119,7 +119,11 @@ class BatchSolver {
     TransferArgs tr;  // to the next coarser level
   };
 
-  BatchSolver(Arena &arena, cudaStream_t stream, const b200ms_options &opt) : arena_(arena), st_(stream), opt_(opt) {}
+  BatchSolver(Arena &arena, cudaStream_t stream, const b200ms_options &opt) : arena_(arena), st_(stream), opt_(opt) {
+    int dev = 0;
+    CUDA_CHECK(cudaGetDevice(&dev));
+    CUDA_CHECK(cudaDeviceGetAttribute(&sms_, cudaDevAttrMultiProcessorCount, dev));
+  }
 
   int B = 0, nx = 0, ny = 0, k = 0, m = 0, restart = 0, nf = 3;
   size_t N = 0, len = 0, vstride = 0, lenE = 0, vsE = 0;
@@ -468,7 +472,7 @@ class BatchSolver {
       if (rows32 && opt_.stencil_variant != 2 && opt_.stencil_variant != 3) {
         // wave quantisation: 7 CTAs of 128 threads per SM are resident; when 32-row CTAs leave the last wave mostly empty
         // (e.g. 32 problems of 512^2: 2.47 waves) 16-row CTAs fill it at the price of 9 % more halo rows
-        const double per_wave = 148.0 * 7.0;
+        const double per_wave = sms_ * 7.0;
         const double c32 = (double)((v.ny + kMarchOut - 1) / kMarchOut) * ((v.nx + 31) / 32) * B / per_wave;
         const double c16 = (double)((v.ny + kMarchOut - 1) / kMarchOut) * ((v.nx + 15) / 16) * B / per_wave;
         const double t32 = std::ceil(c32) * 35.0, t16 = std::ceil(c16) * 19.0;  // waves x row steps per CTA
@@ -542,13 +546,11 @@ class BatchSolver {
     const long key = ((long)md * 32 + p.id) * 1024 + W;
     auto it = m2_resident_.find(key);
     if (it == m2_resident_.end()) {
-      int per_sm = 0, dev = 0, sms = 148;
+      int per_sm = 0;
       if (p.stages > 0)
         CUDA_CHECK(cudaFuncSetAttribute(p.fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)march2_smem(p, kM2MaxW)));
       CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, p.fn, W, march2_smem(p, W)));
-      CUDA_CHECK(cudaGetDevice(&dev));
-      CUDA_CHECK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-      it = m2_resident_.emplace(key, std::max(1, per_sm) * sms).first;
+      it = m2_resident_.emplace(key, std::max(1, per_sm) * sms_).first;
     }
     return it->second;
   }
@@ -1155,11 +1157,11 @@ class BatchSolver {
   static bool vec_ok(size_t ln) { return ln % PackTraits<U>::EPV == 0; }
   int gs_chunks(size_t ln) const {
     const size_t packs = std::max<size_t>(1, ln / 2);
-    return (int)std::max<size_t>(1, std::min<size_t>({(size_t)kDotChunks, packs / 1024 + 1, (size_t)(1184 + B - 1) / B}));
+    return (int)std::max<size_t>(1, std::min<size_t>({(size_t)kDotChunks, packs / 1024 + 1, (size_t)(sms_ * 8 + B - 1) / B}));
   }
   // CTAs per problem for the streaming kernels with a reduction prologue (scale, ir_begin, ir_update): ~8 per SM in total
   int stream_blocks(size_t ln) const {
-    return (int)std::max<size_t>(1, std::min<size_t>({(size_t)256, ln / 2048 + 1, (size_t)(148 * 8 + B - 1) / B}));
+    return (int)std::max<size_t>(1, std::min<size_t>({(size_t)256, ln / 2048 + 1, (size_t)(sms_ * 8 + B - 1) / B}));
   }
   template <typename U>
   U *gpart(int region) { return reinterpret_cast<U *>(gpart_) + (size_t)region * B * kDotChunks * pstride(); }
@@ -1969,6 +1971,7 @@ class BatchSolver {
   cplx *tcoef_ = nullptr;
   std::vector<cd> sig_mg_host_;
   bool dinv_ready_ = false;
+  int sms_ = 0;  // streaming multiprocessors of the device
   std::map<long, int> m2_resident_;  // pair-marching kernel: resident CTAs on the device per (mode, prefetch depth, CTA width)
   cudaGraphExec_t graph_exec_ = nullptr;
   P *graph_result_ = nullptr;

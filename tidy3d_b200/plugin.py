@@ -141,7 +141,7 @@ def solve_all_freqs_relative_batched(self, coords, symmetry, basis_fields):
 
 
 def install(batched: bool = True, device_eps: bool = None):
-    """Route ``tidy3d.plugins.mode.ModeSolver`` through the B200 library.  Raises ImportError without tidy3d.
+    """Route ``tidy3d.plugins.mode.ModeSolver`` through the CUDA library.  Raises ImportError without tidy3d.
     ``device_eps=True``: the batched seams describe each plane once by ``section_of`` and let the device rasterise the
     permittivity of every frequency (falls back to ``_solver_eps`` arrays for custom media); ``None`` keeps the setting."""
     import tidy3d.plugins.mode.mode_solver as ms  # noqa: PLC0415
