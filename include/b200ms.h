@@ -29,7 +29,7 @@
 extern "C" {
 #endif
 
-#define B200MS_VERSION 203
+#define B200MS_VERSION 204
 
 /* return codes */
 enum {
@@ -310,13 +310,26 @@ int b200ms_debug_te_terms(const double *e, int px, int py, double angle_theta, d
 int b200ms_debug_post_tables_bounded(const double *coords, int n, int sym, double lo, double hi, int max_points, int *idx, double *wgt,
                                      double *area);
 
-/* ---- device debug hooks (GPU tests compare these against the numpy model) ------------------- */
-/* y = (A - sigma) x on level `level` of the hierarchy of `prob`; x,y complex128 2*nxl*nyl */
+/* ---- device debug hooks (GPU tests compare these against the float64 model, oracle/mg_model.py) ---- */
+/* One device batch of `nprob` problems, built exactly as b200ms_solve_batch builds it (same incidence flags, a shared
+ * medium stored once with batch stride 0).  The problems must be ones b200ms_solve_batch would solve in one device batch:
+ * same shape, num_modes, arithmetic kind, mu, symmetry, bend axis, direction, basis or not, tensorial kind, precision, PEC
+ * masking and angles (else B200MS_ERR_ARG with a message).  The hierarchy geometry is that of problem 0.
+ * in, in2, out: nprob consecutive complex128 (re,im) vectors; in2 may be NULL (zeros).
+ *   what 0, apply: level 0 and mode 0 / 1: the fp64 Krylov-side operator, out = (A - sigma) in  /  in2 - (A - sigma) in
+ *                  (tensorial problems: the 4N first-order operator).  Otherwise the multigrid operator of level `level`
+ *                  in the multigrid precision (mode + 16 selects it on level 0 as well): mode 0 apply, 1 residual,
+ *                  2 stored-diagonal Jacobi sweep (x = in, rhs = in2), 3 omega D^-1 in2, 4 two sweeps from zero on in2.
+ *                  Vectors have 2 nx_l ny_l elements per problem.
+ *   what 1: one preconditioner application out = M^-1 in (the multigrid V-cycle; tensorial: the block preconditioner).
+ *   what 2: out = (A - sigma)^-1 in by the inner solver of the eigen-iteration, to the handle's inner_tol; *iters gets its
+ *           Arnoldi steps, relres[nprob] the final relative residual of every problem. */
+int b200ms_debug_batch(b200ms_handle *h, int nprob, const b200ms_problem *probs, int what, int level, int mode,
+                       const double *in, const double *in2, double *out, int *iters, double *relres);
+/* b200ms_debug_batch with one problem: apply (what 0), V-cycle (what 1), inner solve (what 2) */
 int b200ms_debug_apply(b200ms_handle *h, const b200ms_problem *prob, int level, int mode,
                        const double *x, const double *rhs, double *y);
-/* one multigrid V-cycle z = M^-1 r on the fine level */
 int b200ms_debug_vcycle(b200ms_handle *h, const b200ms_problem *prob, const double *r, double *z);
-/* x = (A - sigma)^-1 b by preconditioned FGMRES; returns iterations and relative residual */
 int b200ms_debug_solve(b200ms_handle *h, const b200ms_problem *prob, const double *b, double *x,
                        int *iters, double *relres);
 

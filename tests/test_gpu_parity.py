@@ -75,6 +75,19 @@ def test_golden_small(name, preset):
     _check_against_golden(name, fields, n, spec, preset)
 
 
+# inner (FGMRES) iterations per shift-invert apply with the library defaults, measured on an H100 80GB HBM3 (400 W limit).
+# The eigenpairs do not depend on the preconditioner, so a multigrid that has gone subtly wrong shows up only here, as more
+# inner iterations (tests/test_gpu_kernels_vs_model.py pins the kernels themselves).
+INNER_PER_APPLY = {"c1_64": 262 / 38, "c3_128": 906 / 62, "c4_128": 1128 / 44, "lossy_48": 353 / 47, "angled_64": 1003 / 100}
+
+
+@pytest.mark.parametrize("name", sorted(INNER_PER_APPLY))
+def test_inner_iterations_per_apply_stay_in_budget(name):
+    _, _, info = _solve(name)
+    assert info["op_applies"] > 0
+    assert info["inner_iters"] / info["op_applies"] <= 1.3 * INNER_PER_APPLY[name], info
+
+
 @pytest.mark.parametrize("preset", ["reference", "tight"])
 @pytest.mark.parametrize("name", LARGE)
 def test_golden_full_size(name, preset):

@@ -1,9 +1,10 @@
 """GPU: the three stencil kernel families of the real fp32 multigrid path compute the same operator -- the one-column marching
-kernel (round 1, itself pinned to the numpy model and, through the solves, to the reference), the pair-marching kernel
-(csrc/march2.cuh) and its TMA row-staging variant (csrc/march2_tma.cuh).  All modes (apply, residual, stored-diagonal sweep, the
-fused first two sweeps), several levels, widths that need one strip / several strips / are not a multiple of four columns
-(register fallback of the TMA variant) / odd (one-column fallback).  The arithmetic is the same expression for expression, so the
-difference is fp32 rounding of the fused-multiply-add contraction at most."""
+kernel, the pair-marching kernel (csrc/march2.cuh) and its TMA row-staging variant (csrc/march2_tma.cuh).  All modes (apply,
+residual, stored-diagonal sweep, the fused first two sweeps), several levels, widths that need one strip / several strips / are
+not a multiple of four columns (register fallback of the TMA variant) / odd (one-column fallback).  The arithmetic is the same
+expression for expression, so the difference is fp32 rounding of the fused-multiply-add contraction at most.  These tests
+compare the device with itself; tests/test_gpu_kernels_vs_model.py pins all three families, and the fp64 multigrid, to the
+float64 model oracle/mg_model.py."""
 import ctypes as C
 
 import numpy as np

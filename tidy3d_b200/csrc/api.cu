@@ -211,6 +211,12 @@ struct MediumKey {
 };
 // kind: 0 real, 1 complex vectors + real fields, 2 all complex
 int kind_of(const ProblemSetup &s) { return !s.is_complex ? 0 : (s.coef_complex ? 2 : 1); }
+// problems with equal keys may share a device batch (the solver takes everything the key holds from problem 0)
+GroupKey group_key(const ProblemSetup &s, const b200ms_problem &p) {
+  return GroupKey{s.nx, s.ny, s.num_modes, kind_of(s), s.has_mu ? 1 : 0, p.symmetry[0], p.symmetry[1],
+                  s.jz_axis, s.direction, s.relative ? 1 : 0, s.tensorial ? (s.eps_complex ? 2 : 1) : 0, p.precision == 1 ? 1 : 0,
+                  s.masked ? 1 : 0, p.angle_theta, p.angle_phi};
+}
 
 inline size_t align256(size_t n) { return (n + 255) & ~size_t(255); }
 
@@ -673,13 +679,13 @@ struct FieldCopy {  // one pending delivery of packed fields: device region -> c
   size_t bytes;
 };
 
-template <typename T, typename C, typename P, typename PC>
-void solve_group(b200ms_handle *h, const std::vector<int> &ids, const Window &W, const b200ms_problem *prob, b200ms_result *res,
-                 unsigned char *out_region, std::vector<FieldCopy> &copies) {
-  // ids index into the window (global problem index = W.i0 + id)
+// The device batch of the window's problems `ids`: their set-ups, their raw-medium references and whether they all share one
+// medium (then one set of coefficient fields serves the whole batch with batch stride 0, as in a frequency sweep).  Used by
+// solve_group and by the device debug hooks, so that the hooks run the batch production runs.
+bool batch_refs(const Window &W, const std::vector<int> &ids, std::vector<const ProblemSetup *> &ps, std::vector<MediumRef> &refs) {
   const int B = (int)ids.size();
-  std::vector<const ProblemSetup *> ps(B);
-  std::vector<MediumRef> refs(B);
+  ps.assign(B, nullptr);
+  refs.assign(B, MediumRef());
   bool share = true;
   for (int b = 0; b < B; ++b) {
     ps[b] = &W.setups[ids[b]];
@@ -688,6 +694,17 @@ void solve_group(b200ms_handle *h, const std::vector<int> &ids, const Window &W,
     if (W.slot[ids[b]] != W.slot[ids[0]]) share = false;
   }
   if (share) refs.resize(1);
+  return share;
+}
+
+template <typename T, typename C, typename P, typename PC>
+void solve_group(b200ms_handle *h, const std::vector<int> &ids, const Window &W, const b200ms_problem *prob, b200ms_result *res,
+                 unsigned char *out_region, std::vector<FieldCopy> &copies) {
+  // ids index into the window (global problem index = W.i0 + id)
+  const int B = (int)ids.size();
+  std::vector<const ProblemSetup *> ps;
+  std::vector<MediumRef> refs;
+  const bool share = batch_refs(W, ids, ps, refs);
   BatchSolver<T, C, P, PC> S(h->arena, h->stream, h->opt);
   auto wall0 = std::chrono::steady_clock::now();
   S.single_out_ = prob[W.i0 + ids[0]].precision == 1;
@@ -917,10 +934,7 @@ extern "C" int b200ms_solve_batch(b200ms_handle *h, int nprob, const b200ms_prob
             }
             continue;
           }
-          GroupKey key{s.nx, s.ny, s.num_modes, kind_of(s), s.has_mu ? 1 : 0, prob[i].symmetry[0], prob[i].symmetry[1],
-                       s.jz_axis, s.direction, s.relative ? 1 : 0, s.tensorial ? (s.eps_complex ? 2 : 1) : 0, prob[i].precision == 1 ? 1 : 0,
-                       s.masked ? 1 : 0, prob[i].angle_theta, prob[i].angle_phi};
-          groups[key].push_back(q);
+          groups[group_key(s, prob[i])].push_back(q);
           out_bytes += align256((size_t)6 * s.nx * s.ny * s.num_modes * (prob[i].precision == 1 ? 8 : 16));
         }
         DevBuf &ob = h->out[wi & 1];  // last read by the delivery of window wi-2, which has completed (see below)
@@ -1255,13 +1269,35 @@ extern "C" int b200ms_debug_post_tables_bounded(const double *coords, int n, int
 
 // ---- device debug hooks -------------------------------------------------------------------------------
 namespace {
+// host (re,im) pairs of nprob consecutive vectors of n elements <-> the device batch layout (problem b at offset b * n)
+template <typename U>
+void debug_upload(const double *in, size_t n, U *dst) {
+  std::vector<U> a(n);
+  for (size_t e = 0; e < n; ++e) a[e] = in ? from_cd<U>(cd(in[2 * e], in[2 * e + 1])) : zero_of<U>();
+  CUDA_CHECK(cudaMemcpy(dst, a.data(), n * sizeof(U), cudaMemcpyHostToDevice));
+}
+template <typename U>
+void debug_download(const U *src, size_t n, double *out) {
+  std::vector<U> o(n);
+  CUDA_CHECK(cudaMemcpy(o.data(), src, n * sizeof(U), cudaMemcpyDeviceToHost));
+  for (size_t e = 0; e < n; ++e) {
+    const cd v = to_cd(o[e]);
+    out[2 * e] = v.real();
+    out[2 * e + 1] = v.imag();
+  }
+}
+
 template <typename T, typename C, typename P, typename PC>
 int debug_run(b200ms_handle *h, const Window &W, int what, int level, int mode, const double *in0, const double *in1,
               double *out, int *iters, double *relres) {
-  std::vector<const ProblemSetup *> ps(1, &W.setups[0]);
-  std::vector<MediumRef> refs(1, W.refs[0]);
+  const int B = W.i1 - W.i0;
+  std::vector<int> ids(B);
+  for (int b = 0; b < B; ++b) ids[b] = b;
+  std::vector<const ProblemSetup *> ps;
+  std::vector<MediumRef> refs;
+  const bool share = batch_refs(W, ids, ps, refs);
   BatchSolver<T, C, P, PC> S(h->arena, h->stream, h->opt);
-  S.build(ps, false, upload_refs(h, refs, h->stream));
+  S.build(ps, share, upload_refs(h, refs, h->stream));
   if (what == 0 && mode >= 16) {  // mode + 16: the multigrid operator (preconditioner precision) also on level 0
     mode -= 16;
     if (level == 0 && mode != 3) level = -1000;
@@ -1269,70 +1305,64 @@ int debug_run(b200ms_handle *h, const Window &W, int what, int level, int mode, 
   if (what == 0 && (level > 0 || level == -1000 || mode == 3)) {  // multigrid operator of level `level` in preconditioner precision
     if (level == -1000) level = 0;
     if (level < 0 || level >= (int)S.lv.size()) return B200MS_ERR_ARG;
-    const size_t n2 = 2 * S.lv[level].N;
-    std::vector<P> a(n2), b(n2), o(n2);
-    for (size_t e = 0; e < n2; ++e) {
-      a[e] = from_cd<P>(cd(in0[2 * e], in0[2 * e + 1]));
-      b[e] = in1 ? from_cd<P>(cd(in1[2 * e], in1[2 * e + 1])) : zero_of<P>();
-    }
+    const size_t n2 = (size_t)B * 2 * S.lv[level].N;
     P *d0 = reinterpret_cast<P *>(S.basis0()), *d1 = d0 + S.vstride, *d2 = d0 + 2 * S.vstride;
-    CUDA_CHECK(cudaMemcpy(d0, a.data(), n2 * sizeof(P), cudaMemcpyHostToDevice));
-    CUDA_CHECK(cudaMemcpy(d1, b.data(), n2 * sizeof(P), cudaMemcpyHostToDevice));
+    debug_upload<P>(in0, n2, d0);
+    debug_upload<P>(in1, n2, d1);
     if (mode == 3) S.jacobi0(level, d1, d2);
     else S.apply(level, mode, d0, d1, d2);
     CUDA_CHECK(cudaStreamSynchronize(h->stream));
     CUDA_CHECK(cudaGetLastError());
-    CUDA_CHECK(cudaMemcpy(o.data(), d2, n2 * sizeof(P), cudaMemcpyDeviceToHost));
-    for (size_t e = 0; e < n2; ++e) {
-      cd v = to_cd(o[e]);
-      out[2 * e] = v.real();
-      out[2 * e + 1] = v.imag();
-    }
+    debug_download<P>(d2, n2, out);
     return B200MS_OK;
   }
-  if (level < 0 || level >= (int)S.lv.size()) return B200MS_ERR_ARG;
-  const size_t n2 = what == 0 ? 2 * S.lv[level].N : S.len;
-  std::vector<T> a(n2), b(n2);
-  for (size_t e = 0; e < n2; ++e) {
-    a[e] = from_cd<T>(cd(in0[2 * e], in0[2 * e + 1]));
-    b[e] = in1 ? from_cd<T>(cd(in1[2 * e], in1[2 * e + 1])) : zero_of<T>();
-  }
+  if (level != 0) return B200MS_ERR_ARG;
+  const size_t n2 = (size_t)B * S.len;
   T *d0 = S.basis0(), *d1 = S.basis0() + S.vstride, *d2 = S.basis0() + 2 * S.vstride;
-  CUDA_CHECK(cudaMemcpy(d0, a.data(), n2 * sizeof(T), cudaMemcpyHostToDevice));
-  CUDA_CHECK(cudaMemcpy(d1, b.data(), n2 * sizeof(T), cudaMemcpyHostToDevice));
+  debug_upload<T>(in0, n2, d0);
+  debug_upload<T>(in1, n2, d1);
   if (what == 0) {
     S.apply_true(mode, d0, d1, d2);
   } else if (what == 1) {
     S.precondition(d0, d2);
   } else {
     int it = 0;
-    double rr = S.fgmres(d0, d2, it);
+    std::vector<double> rr;
+    S.solve_op(d0, d2, it, nullptr, nullptr, &rr);
     if (iters) *iters = it;
-    if (relres) *relres = rr;
+    if (relres)
+      for (int b = 0; b < B; ++b) relres[b] = rr[b];
   }
   CUDA_CHECK(cudaStreamSynchronize(h->stream));
   CUDA_CHECK(cudaGetLastError());
-  std::vector<T> o(n2);
-  CUDA_CHECK(cudaMemcpy(o.data(), d2, n2 * sizeof(T), cudaMemcpyDeviceToHost));
-  for (size_t e = 0; e < n2; ++e) {
-    cd v = to_cd(o[e]);
-    out[2 * e] = v.real();
-    out[2 * e + 1] = v.imag();
-  }
+  debug_download<T>(d2, n2, out);
   return B200MS_OK;
 }
 
-int debug_dispatch(b200ms_handle *h, const b200ms_problem *prob, int what, int level, int mode, const double *in0,
+int debug_dispatch(b200ms_handle *h, int nprob, const b200ms_problem *prob, int what, int level, int mode, const double *in0,
                    const double *in1, double *out, int *iters, double *relres) {
-  if (!h || !prob || !in0 || !out) return B200MS_ERR_ARG;
+  if (!h || nprob < 1 || !prob || !in0 || !out || what < 0 || what > 2) return B200MS_ERR_ARG;
   if (cudaSetDevice(h->device) != cudaSuccess) return B200MS_ERR_CUDA;
+  h->err.clear();
   try {
     Window W;
-    prepare_window(h, prob, 0, 1, h->raw[0], h->stream, W);
+    prepare_window(h, prob, 0, nprob, h->raw[0], h->stream, W);
+    for (const ProblemSetup &s : W.setups)
+      if (s.status != B200MS_OK) {
+        h->err = s.error;
+        return s.status;
+      }
+    // one device batch, formed only where b200ms_solve_batch would form it: the same group key for every problem
     const ProblemSetup &s = W.setups[0];
-    if (s.status != B200MS_OK) {
-      h->err = s.error;
-      return s.status;
+    const GroupKey k0 = group_key(s, prob[0]);
+    for (int q = 1; q < nprob; ++q) {
+      const GroupKey kq = group_key(W.setups[q], prob[q]);
+      if (k0 < kq || kq < k0) {
+        h->err = "b200ms_debug_batch: problem " + std::to_string(q) +
+                 " differs from problem 0 in what b200ms_solve_batch groups by (shape, modes, arithmetic kind, mu, symmetry, bend axis, "
+                 "direction, basis, tensorial kind, precision, PEC masking, angles)";
+        return B200MS_ERR_ARG;
+      }
     }
     const bool f32 = h->opt.mg_precision == 1;
     switch (kind_of(s)) {
@@ -1353,14 +1383,18 @@ int debug_dispatch(b200ms_handle *h, const b200ms_problem *prob, int what, int l
 }
 }  // namespace
 
+extern "C" int b200ms_debug_batch(b200ms_handle *h, int nprob, const b200ms_problem *probs, int what, int level, int mode,
+                                  const double *in, const double *in2, double *out, int *iters, double *relres) {
+  return debug_dispatch(h, nprob, probs, what, level, mode, in, in2, out, iters, relres);
+}
 extern "C" int b200ms_debug_apply(b200ms_handle *h, const b200ms_problem *prob, int level, int mode, const double *x,
                                   const double *rhs, double *y) {
-  return debug_dispatch(h, prob, 0, level, mode, x, rhs, y, nullptr, nullptr);
+  return debug_dispatch(h, 1, prob, 0, level, mode, x, rhs, y, nullptr, nullptr);
 }
 extern "C" int b200ms_debug_vcycle(b200ms_handle *h, const b200ms_problem *prob, const double *r, double *z) {
-  return debug_dispatch(h, prob, 1, 0, 0, r, nullptr, z, nullptr, nullptr);
+  return debug_dispatch(h, 1, prob, 1, 0, 0, r, nullptr, z, nullptr, nullptr);
 }
 extern "C" int b200ms_debug_solve(b200ms_handle *h, const b200ms_problem *prob, const double *b, double *x, int *iters,
                                   double *relres) {
-  return debug_dispatch(h, prob, 2, 0, 0, b, nullptr, x, iters, relres);
+  return debug_dispatch(h, 1, prob, 2, 0, 0, b, nullptr, x, iters, relres);
 }

@@ -1,293 +1,17 @@
 """DEV TOOL (not product, not oracle): numpy model of the GPU algorithm, used to settle the numerical
-design before writing CUDA -- matrix-free operator, PML-aware semi-coarsening multigrid, FGMRES inner
-solve and shift-invert Krylov-Schur outer iteration.  Mirrors tidy3d_b200/csrc one-to-one so that the
-CUDA path can be debugged against it component by component.
+design before writing CUDA -- FGMRES inner solve and shift-invert Krylov-Schur outer iteration.  The
+matrix-free operator and the PML-aware semi-coarsening multigrid are those of oracle/mg_model.py (the
+float64 model the GPU tests pin the kernels to); they are re-exported here.
 """
 from __future__ import annotations
 
+import os
+import sys
+
 import numpy as np
 
-
-# ------------------------------------------------------------------------------------------------
-# level = one grid of the hierarchy
-# ------------------------------------------------------------------------------------------------
-class Level:
-    """Operator data on one tensor-product grid.
-
-    lens[ax] = (Lf, Lb): complex-stretched primal/dual lengths * k0 (dimensionless).
-    pmc[ax]: PMC at the min wall.  fields: exx, eyy, iez (1/ezz), mxx, myy, imz (1/mzz) as (nx, ny).
-    pos[ax]: real node coordinates (n+1) used only for interpolation weights.
-    """
-
-    def __init__(self, nx, ny, lens, pmc, fields, pos, sigma):
-        self.nx, self.ny = nx, ny
-        self.lens, self.pmc, self.pos, self.sigma = lens, pmc, pos, sigma
-        self.exx, self.eyy, self.iez, self.mxx, self.myy, self.imz = fields
-        self.coef = [self._coeffs(n, *lens[ax], pmc[ax]) for ax, n in enumerate((nx, ny))]
-        self.diag = self._diagonal() - sigma
-
-    @staticmethod
-    def _coeffs(n, lf, lb, pmc):
-        f0 = np.zeros(n, complex); f1 = np.zeros(n, complex)
-        b0 = np.zeros(n, complex); bm = np.zeros(n, complex)
-        if n > 1:
-            f0[:] = -1 / lf; f1[:-1] = 1 / lf[:-1]
-            if not pmc:
-                f0[0] = 0
-            b0[:] = 1 / lb; bm[1:] = -1 / lb[1:]
-            b0[0] = 2 / lb[0] if pmc else 0
-        return f0, f1, b0, bm
-
-    # -- shifted operator (A - sigma) v, v shape (2, nx, ny) ------------------------------------
-    def apply(self, v, shifted=True):
-        (xf0, xf1, xb0, xbm), (yf0, yf1, yb0, ybm) = self.coef
-        v1, v2 = v[0], v[1]
-        # t at Hz sites
-        t = xf0[:, None] * v2 - yf0[None, :] * v1
-        t[:-1] += xf1[:-1, None] * v2[1:]
-        t[:, :-1] -= yf1[None, :-1] * v1[:, 1:]
-        t *= self.imz
-        # u at Ez sites:  u = -(Dxb(exx v1) + Dyb(eyy v2)) / ezz
-        a, b = self.exx * v1, self.eyy * v2
-        u = xb0[:, None] * a + yb0[None, :] * b
-        u[1:] += xbm[1:, None] * a[:-1]
-        u[:, 1:] += ybm[None, 1:] * b[:, :-1]
-        u *= -self.iez
-        p1 = xf0[:, None] * u
-        p1[:-1] += xf1[:-1, None] * u[1:]
-        dybt = yb0[None, :] * t
-        dybt[:, 1:] += ybm[None, 1:] * t[:, :-1]
-        p1 += self.myy * (dybt - a)
-        p2 = yf0[None, :] * u
-        p2[:, :-1] += yf1[None, :-1] * u[:, 1:]
-        dxbt = xb0[:, None] * t
-        dxbt[1:] += xbm[1:, None] * t[:-1]
-        p2 -= self.mxx * (dxbt + b)
-        out = np.stack((p1, p2))
-        if shifted:
-            out -= self.sigma * v
-        return out
-
-    def _diagonal(self):
-        (xf0, xf1, xb0, xbm), (yf0, yf1, yb0, ybm) = self.coef
-        iez, imz = self.iez, self.imz
-        nx, ny = self.nx, self.ny
-        z = lambda: np.zeros((nx, ny), complex)
-        s = z(); s += (xf0 * xb0)[:, None] * iez; s[:-1] += (xf1[:-1] * xbm[1:])[:, None] * iez[1:]
-        d1 = -self.exx * s
-        s = z(); s += (yb0 * yf0)[None, :] * imz; s[:, 1:] += (ybm[1:] * yf1[:-1])[None, :] * imz[:, :-1]
-        d1 += -self.myy * s - self.myy * self.exx
-        s = z(); s += (yf0 * yb0)[None, :] * iez; s[:, :-1] += (yf1[:-1] * ybm[1:])[None, :] * iez[:, 1:]
-        d2 = -self.eyy * s
-        s = z(); s += (xb0 * xf0)[:, None] * imz; s[1:] += (xbm[1:] * xf1[:-1])[:, None] * imz[:-1]
-        d2 += -self.mxx * s - self.mxx * self.eyy
-        return np.stack((d1, d2))
-
-
-# ------------------------------------------------------------------------------------------------
-# 1-D aggregation + transfer operators
-# ------------------------------------------------------------------------------------------------
-def aggregate_1d(lf, H, slack=1.25, max_cells=3):
-    """Greedy aggregation of neighbouring cells: grow an aggregate while its |stretched length|
-    stays <= slack*H (at most `max_cells` cells).  Returns start indices a[0..nc] (a[nc] = n)."""
-    n = len(lf)
-    ell = np.abs(lf)
-    starts = []
-    i = 0
-    while i < n:
-        starts.append(i)
-        tot = ell[i]; cnt = 1
-        while i + cnt < n and cnt < max_cells and tot + ell[i + cnt] <= slack * H:
-            tot += ell[i + cnt]; cnt += 1
-            if cnt >= 2 and tot >= 0.75 * H:
-                break
-        i += cnt
-    starts.append(n)
-    return np.array(starts)
-
-
-def interp_node(a, pos):
-    """Fine node i -> (I0, w0, I1, w1).  Coarse node I sits on fine node a[I]; beyond the last
-    coarse node we interpolate towards the (zero) max wall."""
-    nc = len(a) - 1
-    n = a[-1]
-    out = np.zeros((n, 2), int); w = np.zeros((n, 2))
-    for I in range(nc):
-        x0 = pos[a[I]]; x1 = pos[a[I + 1]]
-        for i in range(a[I], a[I + 1]):
-            t = (pos[i] - x0) / (x1 - x0)
-            out[i] = (I, min(I + 1, nc - 1)); w[i] = (1 - t, t if I + 1 < nc else 0.0)
-    return out, w
-
-
-def interp_edge(a, pos):
-    """Fine cell i -> two coarse cells by linear interpolation between coarse cell centres."""
-    nc = len(a) - 1
-    n = a[-1]
-    xc = 0.5 * (pos[:-1] + pos[1:])
-    Xc = np.array([0.5 * (pos[a[I]] + pos[a[I + 1]]) for I in range(nc)])
-    out = np.zeros((n, 2), int); w = np.zeros((n, 2))
-    for I in range(nc):
-        for i in range(a[I], a[I + 1]):
-            if xc[i] < Xc[I] and I > 0:
-                t = (xc[i] - Xc[I - 1]) / (Xc[I] - Xc[I - 1]); out[i] = (I - 1, I); w[i] = (1 - t, t)
-            elif xc[i] > Xc[I] and I + 1 < nc:
-                t = (xc[i] - Xc[I]) / (Xc[I + 1] - Xc[I]); out[i] = (I, I + 1); w[i] = (1 - t, t)
-            else:
-                out[i] = (I, I); w[i] = (1.0, 0.0)
-    return out, w
-
-
-def dense_1d(idx, w, nc):
-    n = len(idx)
-    P = np.zeros((n, nc))
-    for i in range(n):
-        P[i, idx[i, 0]] += w[i, 0]; P[i, idx[i, 1]] += w[i, 1]
-    return P
-
-
-class Transfer:
-    """Tensor-product prolongation / restriction between two levels (dense 1-D factors; the CUDA
-    version stores the same thing as per-row (index, weight) pairs)."""
-
-    def __init__(self, ax_aggr, pos, pmc=(False, False)):
-        self.pmc = pmc
-        (ax, ay), (px, py) = ax_aggr, pos
-        ncx, ncy = len(ax) - 1, len(ay) - 1
-        self.Pxn = dense_1d(*interp_node(ax, px), ncx); self.Pxe = dense_1d(*interp_edge(ax, px), ncx)
-        self.Pyn = dense_1d(*interp_node(ay, py), ncy); self.Pye = dense_1d(*interp_edge(ay, py), ncy)
-        nrm = lambda P: (P / np.maximum(P.sum(0), 1e-300)).T  # rows of R sum to one
-        self.Rxn, self.Rxe, self.Ryn, self.Rye = nrm(self.Pxn), nrm(self.Pxe), nrm(self.Pyn), nrm(self.Pye)
-
-    def prolong(self, c):  # Ex: x-edge,y-node ; Ey: x-node,y-edge
-        out = np.stack((self.Pxe @ c[0] @ self.Pyn.T, self.Pxn @ c[1] @ self.Pye.T))
-        # PEC min walls: the tangential wall unknowns form a decoupled block; keep them exactly zero
-        if not self.pmc[1] and out.shape[2] > 1:
-            out[0][:, 0] = 0
-        if not self.pmc[0] and out.shape[1] > 1:
-            out[1][0, :] = 0
-        return out
-
-    def restrict(self, f):
-        out = np.stack((self.Rxe @ f[0] @ self.Ryn.T, self.Rxn @ f[1] @ self.Rye.T))
-        if not self.pmc[1] and out.shape[2] > 1:
-            out[0][:, 0] = 0
-        if not self.pmc[0] and out.shape[1] > 1:
-            out[1][0, :] = 0
-        return out
-
-    # coefficient fields by site type
-    def avg(self, f, xt, yt):
-        Rx = self.Rxe if xt == "e" else self.Rxn
-        Ry = self.Rye if yt == "e" else self.Ryn
-        return Rx @ f @ Ry.T
-
-
-def coarsen(lv: Level, H):
-    ax = aggregate_1d(lv.lens[0][0], H) if lv.nx > 1 else np.array([0, 1])
-    ay = aggregate_1d(lv.lens[1][0], H) if lv.ny > 1 else np.array([0, 1])
-    ncx, ncy = len(ax) - 1, len(ay) - 1
-    if ncx == lv.nx and ncy == lv.ny:
-        return None, None
-    tr = Transfer((ax, ay), lv.pos, lv.pmc)
-    lens = []
-    for a, (lf, lb) in zip((ax, ay), lv.lens):
-        Lf = np.add.reduceat(lf, a[:-1])
-        Lb = np.empty_like(Lf); Lb[0] = Lf[0]; Lb[1:] = 0.5 * (Lf[:-1] + Lf[1:])
-        lens.append((Lf, Lb))
-    pos = [lv.pos[0][ax], lv.pos[1][ay]]
-    fields = (
-        tr.avg(lv.exx, "e", "n"), tr.avg(lv.eyy, "n", "e"), 1 / tr.avg(1 / lv.iez, "n", "n"),
-        tr.avg(lv.mxx, "n", "e"), tr.avg(lv.myy, "e", "n"), 1 / tr.avg(1 / lv.imz, "e", "e"),
-    )
-    return Level(ncx, ncy, lens, lv.pmc, fields, pos, lv.sigma), tr
-
-
-def fine_level(st, sigma):
-    """Build level 0 from oracle.restatement.setup() output (diagonal case)."""
-    nx, ny, k0 = st["nx"], st["ny"], st["k0"]
-    e, m = st["eps"], st["mu"]
-    g = lambda a: a.reshape(nx, ny)
-    lens = [(lf * k0, lb * k0) for lf, lb in st["slen"]]
-    fields = (g(e[0, 0]), g(e[1, 1]), 1 / g(e[2, 2]), g(m[0, 0]), g(m[1, 1]), 1 / g(m[2, 2]))
-    return Level(nx, ny, lens, st["pmc"], fields, st["new_coords"], sigma)
-
-
-# ------------------------------------------------------------------------------------------------
-# multigrid preconditioner
-# ------------------------------------------------------------------------------------------------
-class Multigrid:
-    def __init__(self, lv0, min_size=12, max_levels=10, nu=2, omega=0.8, coarse_sweeps=40, ratio=1.5,
-                 smoother="jacobi", cheb_deg=3, lam_max=2.0, lam_frac=4.0, exact_coarse=False, coarse_gmres=0, kh_limit=0.0, kmax=0.0):
-        self.exact_coarse = exact_coarse; self._lu = None; self.coarse_gmres = coarse_gmres
-        self.levels, self.tr = [lv0], []
-        h0 = min(np.abs(l[0]).min() for l, n in zip(lv0.lens, (lv0.nx, lv0.ny)) if n > 1)
-        H = h0
-        while len(self.levels) < max_levels and max(self.levels[-1].nx, self.levels[-1].ny) > min_size:
-            H *= 2
-            if kh_limit and kmax * H > kh_limit:
-                break
-            c, tr = coarsen(self.levels[-1], H)
-            if c is None:
-                continue
-            self.levels.append(c); self.tr.append(tr)
-        self.nu, self.omega, self.coarse_sweeps = nu, omega, coarse_sweeps
-        self.smoother, self.cheb_deg, self.lam_max, self.lam_frac = smoother, cheb_deg, lam_max, lam_frac
-        self.applies = 0.0  # fine-grid-apply equivalents
-
-    def _smooth(self, lv, x, b, n, zero_init=False):
-        w = lv.nx * lv.ny / (self.levels[0].nx * self.levels[0].ny)
-        if self.smoother == "jacobi":
-            for k in range(n):
-                if zero_init and k == 0:
-                    x = self.omega * b / lv.diag
-                else:
-                    x = x + self.omega * (b - lv.apply(x)) / lv.diag; self.applies += w
-            return x
-        # Chebyshev on D^-1 A over [lam_max/lam_frac, lam_max], n passes of degree cheb_deg
-        lmax, lmin = self.lam_max, self.lam_max / self.lam_frac
-        theta, delta = 0.5 * (lmax + lmin), 0.5 * (lmax - lmin)
-        for k in range(n):
-            r = b / lv.diag if (zero_init and k == 0) else (b - lv.apply(x)) / lv.diag
-            if not (zero_init and k == 0):
-                self.applies += w
-            sig = theta / delta; rho = 1 / sig
-            d = r / theta
-            x = x + d if not (zero_init and k == 0) else d
-            for _ in range(self.cheb_deg - 1):
-                r = r - lv.apply(d) / lv.diag; self.applies += w
-                rho_new = 1 / (2 * sig - rho)
-                d = rho_new * rho * d + 2 * rho_new / delta * r
-                x = x + d; rho = rho_new
-        return x
-
-    def vcycle(self, b, l=0):
-        lv = self.levels[l]
-        if l == len(self.levels) - 1 and self.exact_coarse:
-            if self._lu is None:
-                import scipy.linalg as sl
-                nn = 2 * lv.nx * lv.ny
-                M = np.zeros((nn, nn), complex)
-                for k in range(nn):
-                    e = np.zeros(nn, complex); e[k] = 1
-                    M[:, k] = lv.apply(e.reshape(2, lv.nx, lv.ny)).ravel()
-                self._lu = sl.lu_factor(M)
-            import scipy.linalg as sl
-            return sl.lu_solve(self._lu, b.ravel()).reshape(b.shape)
-        if l == len(self.levels) - 1 and self.coarse_gmres:
-            x, its, res = fgmres(lv.apply, lambda r: r / lv.diag, b, tol=1e-3, restart=self.coarse_gmres, maxit=self.coarse_gmres)
-            self.applies += its * lv.nx * lv.ny / (self.levels[0].nx * self.levels[0].ny)
-            return x
-        if l == len(self.levels) - 1:
-            return self._smooth(lv, None, b, self.coarse_sweeps, zero_init=True)
-        x = self._smooth(lv, None, b, self.nu, zero_init=True)
-        r = b - lv.apply(x); self.applies += lv.nx * lv.ny / (self.levels[0].nx * self.levels[0].ny)
-        ec = self.vcycle(self.tr[l].restrict(r), l + 1)
-        x = x + self.tr[l].prolong(ec)
-        return self._smooth(lv, x, b, self.nu)
-
-    def __call__(self, b):
-        return self.vcycle(b)
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+from oracle.mg_model import Level, Multigrid, Opts, Problem, Transfer, aggregate_axis, plan_hierarchy  # noqa: E402,F401
 
 
 # ------------------------------------------------------------------------------------------------
