@@ -29,7 +29,7 @@
 extern "C" {
 #endif
 
-#define B200MS_VERSION 204
+#define B200MS_VERSION 205
 
 /* return codes */
 enum {
@@ -89,6 +89,10 @@ typedef struct {
   const unsigned short *site_medium; /* NULL, or 3*nx*ny medium indices [Ex sites | Ey sites | Ez sites], each C-order with y fastest:
                               the medium found at every Yee site before the listed shapes are drawn (replaces "background
                               everywhere").  Indices >= nmedia are a caller error (clamped to nmedia - 1 on the device) */
+  /* ---- since version 205 ---- */
+  const double *deps_table; /* NULL (nondispersive media), or nmedia x 9 complex128 (re,im): d eps / df (1/Hz) of each medium at this
+                              problem's frequency, rasterised like eps_table; only the material term of result.dn_dfreq reads it
+                              (diagonal components) */
 } b200ms_section;
 
 /* One eigenproblem == one compute_modes call (one plane, one frequency). */
@@ -134,6 +138,8 @@ typedef struct {
                             The trapezoid weights of flux, TE fraction and modal overlaps are then truncated to the part of each
                             cell the plane covers, like the reference's _diff_area (monitor_data.py:437-455: mid-points and end
                             points clipped to monitor.bounds).  Only the post-processing results depend on it */
+  const double *eps_dfreq; /* since version 205.  NULL (nondispersive medium), or d eps_cross / df (1/Hz) in the layout of `eps`; only the
+                            diagonal components are read, and only by the material term of result.dn_dfreq */
 } b200ms_problem;
 
 typedef struct {
@@ -165,6 +171,15 @@ typedef struct {
                             was in, operator data already resident in HBM, results still on the device */
   double total_ms;       /* out: host wall time of that batch incl. upload of the operator and download of the fields */
   double max_residual;   /* out: max_i ||A v_i - lambda_i v_i|| / (|lambda_i| ||v_i||) */
+  /* ---- since version 205: first-order derivatives of each mode from its own solve (left eigenvector w = G J Q v, see DESIGN.md §4).
+     Diagonal problems only (PML, bend, lossy, both wall types, diagonal mu); asking for them on a tensorial, relative or
+     removed-PEC-unknown problem sets status B200MS_ERR_UNSUPPORTED.  They do not change which problems share a device batch,
+     nor n_complex or the fields ---- */
+  double *dn_dfreq;      /* NULL, or caller-allocated num_modes complex128 (re,im): d(n_eff + i k_eff)/df (1/Hz), including the material
+                            dispersion given by problem.eps_dfreq / section.deps_table.  Group index: n_g = n_eff + f Re(dn/df) */
+  double *dn_deps;       /* NULL, or caller-allocated 3*nx*ny*num_modes complex128 (re,im), [xx|yy|zz][ix][iy][mode]: d(n_eff + i k_eff)
+                            / d eps_aa of the caller's eps_cross at the Ex / Ey / Ez site of each cell (PML stretch held fixed; 0 at
+                            PEC-valued cells); HOST or DEVICE memory like `fields` */
 } b200ms_result;
 
 /* Tunables (all have defaults; see DESIGN.md). */

@@ -17,7 +17,7 @@ import numpy as np
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("B200MS_LIB") or os.path.join(_HERE, "libb200ms.so")  # B200MS_LIB: developer override (A/B of builds)
 
-ABI_VERSION = 204  # B200MS_VERSION of include/b200ms.h
+ABI_VERSION = 205  # B200MS_VERSION of include/b200ms.h
 OK, ERR_SHAPE, ERR_NO_MODES, ERR_UNSUPPORTED, ERR_CUDA, ERR_NOCONV, ERR_ARG = range(7)
 SPEC_NAMES = {0: "diagonal", 1: "tensorial_real", 2: "tensorial_complex"}
 
@@ -27,7 +27,7 @@ _ip = C.POINTER(C.c_int)
 
 class SectionStruct(C.Structure):
     _fields_ = [("nrect", C.c_int), ("rects", _dp), ("medium", _ip), ("nmedia", C.c_int), ("eps_table", _dp),
-                ("shape", _ip), ("poly_start", _ip), ("poly_xy", _dp), ("site_medium", C.POINTER(C.c_ushort))]
+                ("shape", _ip), ("poly_start", _ip), ("poly_xy", _dp), ("site_medium", C.POINTER(C.c_ushort)), ("deps_table", _dp)]
 
 
 class Problem(C.Structure):
@@ -37,7 +37,7 @@ class Problem(C.Structure):
         ("freq", C.c_double), ("target_neff", C.c_double), ("bend_radius", C.c_double),
         ("angle_theta", C.c_double), ("angle_phi", C.c_double),
         ("eps", _dp), ("coords_x", _dp), ("coords_y", _dp), ("mu", _dp), ("section", C.POINTER(SectionStruct)), ("basis_e", _dp),
-        ("grid_correction", _dp), ("plane_bounds", _dp),
+        ("grid_correction", _dp), ("plane_bounds", _dp), ("eps_dfreq", _dp),
     ]  # fmt: skip
 
 
@@ -46,6 +46,7 @@ class Result(C.Structure):
         ("fields", _dp), ("n_complex", _dp), ("flux", _dp), ("te_fraction", _dp), ("overlap_prev", _dp), ("eps_spec", C.c_int), ("status", C.c_int), ("converged", C.c_int),
         ("outer_iters", C.c_int), ("op_applies", C.c_int), ("inner_iters", C.c_int), ("stencil_applies", C.c_int),
         ("is_complex", C.c_int), ("solve_ms", C.c_double), ("total_ms", C.c_double), ("max_residual", C.c_double),
+        ("dn_dfreq", _dp), ("dn_deps", _dp),
     ]  # fmt: skip
 
 
@@ -132,10 +133,11 @@ class PackedProblem:
     """Owns the contiguous arrays a ``Problem`` struct points to."""
 
     def __init__(self, eps_cross, coords, freq, mode_spec, symmetry=(0, 0), direction="+", eps_packed=None, basis_fields=None,
-                 mu_cross=None, target_override=None, incidence=False, post=0, section=None, grid_correction=None, plane_bounds=None):
+                 mu_cross=None, target_override=None, incidence=False, post=0, section=None, grid_correction=None, plane_bounds=None,
+                 eps_dfreq=None, derivatives=False):
         self.section = None
         if section is not None:  # geometric cross-section rasterised on the device (tidy3d_b200/sections.py); no eps array
-            self.section, self._section_arrays = section.pack(float(freq), (len(coords[0]) - 1, len(coords[1]) - 1))
+            self.section, self._section_arrays = section.pack(float(freq), (len(coords[0]) - 1, len(coords[1]) - 1), dispersion=derivatives)
             eps = None
         elif eps_packed is not None:
             eps = eps_packed
@@ -225,6 +227,14 @@ class PackedProblem:
             if self.plane_bounds.size != 4 or not (self.plane_bounds[0] <= self.plane_bounds[1] and self.plane_bounds[2] <= self.plane_bounds[3]):
                 raise ValueError("plane_bounds must be (xmin, xmax, ymin, ymax)")
             p.plane_bounds = _ptr(self.plane_bounds)
+        self.eps_dfreq = None
+        if eps_dfreq is not None:  # d eps_cross / df in the eps layout (material term of the mode derivatives)
+            if section is not None:
+                raise ValueError("eps_dfreq belongs to an eps_cross problem; a section's media carry their own dispersion")
+            self.eps_dfreq = np.ascontiguousarray(np.stack([np.asarray(eps_dfreq[i], dtype=np.complex128) for i in range(len(eps_dfreq))]))
+            if self.eps_dfreq.shape != (9, self.nx, self.ny):
+                raise ValueError("eps_dfreq must have the nine components and the shape of eps_cross")
+            p.eps_dfreq = _ptr(self.eps_dfreq.view(np.float64))
         self.struct = p
         self.num_modes = p.num_modes
 
@@ -315,21 +325,30 @@ class Handle:
         except Exception:
             pass
 
-    def solve_batch(self, packed, want_fields=True, fields_ptrs=None, want_flux=False, want_overlaps=False):
+    def solve_batch(self, packed, want_fields=True, fields_ptrs=None, want_flux=False, want_overlaps=False, want_dfreq=False, want_deps=False):
         """packed: list of PackedProblem.  Returns (rc, fields list | None, n_complex list, Result structs).
 
         ``fields_ptrs``: optional list of raw addresses (host or DEVICE memory, e.g. ``tensor.data_ptr()``) the library
         writes the fields of each problem to, instead of freshly allocated pinned host arrays; then ``fields`` is None.
-        Fields are complex128, or complex64 for ``precision == "single"`` problems (solver.py:265-267)."""
+        Fields are complex128, or complex64 for ``precision == "single"`` problems (solver.py:265-267).  ``want_dfreq`` /
+        ``want_deps``: d n / df and d n / d eps of every mode (``last_dn_dfreq`` / ``last_dn_deps``)."""
         n = len(packed)
         probs = (Problem * n)(*[p.struct for p in packed])
         results = (Result * n)()
         fields, ncs = [], []
-        self.last_flux, self.last_te, self.last_overlaps = [], [], []
+        self.last_flux, self.last_te, self.last_overlaps, self.last_dn_dfreq, self.last_dn_deps = [], [], [], [], []
         for i, p in enumerate(packed):
             nc = np.zeros(p.num_modes, dtype=np.complex128)
             ncs.append(nc)
             results[i].n_complex = _ptr(nc.view(np.float64))
+            if want_dfreq:
+                d = np.zeros(p.num_modes, dtype=np.complex128)
+                self.last_dn_dfreq.append(d)
+                results[i].dn_dfreq = _ptr(d.view(np.float64))
+            if want_deps:
+                d = np.zeros((3, p.nx, p.ny, p.num_modes), dtype=np.complex128)
+                self.last_dn_deps.append(d)
+                results[i].dn_deps = _ptr(d.view(np.float64))
             if want_flux:
                 fl, te = np.zeros(p.num_modes), np.zeros(p.num_modes)
                 self.last_flux.append(fl)

@@ -17,6 +17,7 @@
 #include "../../include/b200ms.h"
 #include "post.cuh"
 #include "solver.cuh"
+#include "derivatives.cuh"
 
 using namespace b200ms;
 
@@ -60,6 +61,7 @@ struct b200ms_handle {
   DevBuf scan;        // reduction scratch + per-medium results of prepare_window
   DevBuf refs;        // MediumRef array of the batch being built
   DevBuf post;        // interpolation tables / partials / results of the on-device post-processing
+  DevBuf deriv;       // tables, partial sums, dispersion input and d n / d eps map of the derivative pass
   DevBuf warm;        // sorted Ritz vectors of the previous device batch of this call ([k][B][len]): warm start of the next one
   int warm_B = 0, warm_k = 0, warm_tsize = 0;
   size_t warm_len = 0;
@@ -153,6 +155,7 @@ extern "C" int b200ms_destroy(b200ms_handle *h) {
   h->refs.release();
   h->post.release();
   h->warm.release();
+  h->deriv.release();
   if (h->io_stream) cudaStreamDestroy(h->io_stream);
   if (h->dl_stream) cudaStreamDestroy(h->dl_stream);
   if (h->flush_buf) cudaFree(h->flush_buf);
@@ -241,6 +244,31 @@ size_t section_device_bytes(const b200ms_section &sec, int nx, int ny) {
   return b;
 }
 
+// Uploads a geometric cross-section into `cur` (section_device_bytes of space) with `table` as its nmedia x 9 medium table:
+// the permittivity table for the raster of the medium, the d eps / df table for the dispersion input of the derivative pass.
+SectionDev upload_section(const b200ms_section &sec, const b200ms_problem &p, const double *table, unsigned char *cur, cudaStream_t st,
+                          size_t &h2d_bytes) {
+  const size_t N = (size_t)p.nx * p.ny;
+  auto put = [&](const void *src, size_t bytes) -> unsigned char * {  // 256-byte aligned sub-buffer, filled from host memory
+    unsigned char *dst = cur;
+    if (bytes) CUDA_CHECK(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyHostToDevice, st));
+    cur += align256(bytes);
+    h2d_bytes += bytes;
+    return dst;
+  };
+  const int nv = (sec.poly_start && sec.nrect > 0) ? sec.poly_start[sec.nrect] : 0;
+  double *d_rects = reinterpret_cast<double *>(put(sec.rects, (size_t)sec.nrect * 4 * sizeof(double)));
+  int *d_med = reinterpret_cast<int *>(put(sec.medium, (size_t)sec.nrect * sizeof(int)));
+  cplx *d_tab = reinterpret_cast<cplx *>(put(table, (size_t)sec.nmedia * 9 * sizeof(cplx)));
+  double *d_x = reinterpret_cast<double *>(put(p.coords_x, (size_t)(p.nx + 1) * sizeof(double)));
+  double *d_y = reinterpret_cast<double *>(put(p.coords_y, (size_t)(p.ny + 1) * sizeof(double)));
+  const int *d_shape = sec.shape ? reinterpret_cast<const int *>(put(sec.shape, (size_t)sec.nrect * sizeof(int))) : nullptr;
+  const int *d_pstart = nv > 0 ? reinterpret_cast<const int *>(put(sec.poly_start, (size_t)(sec.nrect + 1) * sizeof(int))) : nullptr;
+  const double *d_pxy = nv > 0 ? reinterpret_cast<const double *>(put(sec.poly_xy, (size_t)nv * 2 * sizeof(double))) : nullptr;
+  const unsigned short *d_site = sec.site_medium ? reinterpret_cast<const unsigned short *>(put(sec.site_medium, 3 * N * sizeof(unsigned short))) : nullptr;
+  return SectionDev{sec.nrect, d_rects, d_med, d_tab, d_x, d_y, sec.nmedia, d_shape, d_pstart, d_pxy, d_site};
+}
+
 void prepare_window(b200ms_handle *h, const b200ms_problem *prob, int i0, int i1, DevBuf &raw, cudaStream_t st, Window &W) {
   const int n = i1 - i0;
   W.i0 = i0;
@@ -301,26 +329,7 @@ void prepare_window(b200ms_handle *h, const b200ms_problem *prob, int i0, int i1
       CUDA_CHECK(cudaMemcpyAsync(raw.p + off_eps[q], p.eps, 9 * N * sizeof(cplx), cudaMemcpyDefault, st));
       W.h2d_bytes += 9 * N * sizeof(cplx);
     } else {  // rasterise the geometric cross-section on the device (f-2: replaces nine epsilon_on_grid calls + a 9N upload)
-      const b200ms_section &sec = *p.section;
-      unsigned char *cur = raw.p + off_sec[q];
-      auto put = [&](const void *src, size_t bytes) -> unsigned char * {  // 256-byte aligned sub-buffer, filled from host memory
-        unsigned char *dst = cur;
-        if (bytes) CUDA_CHECK(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyHostToDevice, st));
-        cur += align256(bytes);
-        W.h2d_bytes += bytes;
-        return dst;
-      };
-      const int nv = (sec.poly_start && sec.nrect > 0) ? sec.poly_start[sec.nrect] : 0;
-      double *d_rects = reinterpret_cast<double *>(put(sec.rects, (size_t)sec.nrect * 4 * sizeof(double)));
-      int *d_med = reinterpret_cast<int *>(put(sec.medium, (size_t)sec.nrect * sizeof(int)));
-      cplx *d_tab = reinterpret_cast<cplx *>(put(sec.eps_table, (size_t)sec.nmedia * 9 * sizeof(cplx)));
-      double *d_x = reinterpret_cast<double *>(put(p.coords_x, (size_t)(p.nx + 1) * sizeof(double)));
-      double *d_y = reinterpret_cast<double *>(put(p.coords_y, (size_t)(p.ny + 1) * sizeof(double)));
-      const int *d_shape = sec.shape ? reinterpret_cast<const int *>(put(sec.shape, (size_t)sec.nrect * sizeof(int))) : nullptr;
-      const int *d_pstart = nv > 0 ? reinterpret_cast<const int *>(put(sec.poly_start, (size_t)(sec.nrect + 1) * sizeof(int))) : nullptr;
-      const double *d_pxy = nv > 0 ? reinterpret_cast<const double *>(put(sec.poly_xy, (size_t)nv * 2 * sizeof(double))) : nullptr;
-      const unsigned short *d_site = sec.site_medium ? reinterpret_cast<const unsigned short *>(put(sec.site_medium, 3 * N * sizeof(unsigned short))) : nullptr;
-      SectionDev sd{sec.nrect, d_rects, d_med, d_tab, d_x, d_y, sec.nmedia, d_shape, d_pstart, d_pxy, d_site};
+      SectionDev sd = upload_section(*p.section, p, p.section->eps_table, raw.p + off_sec[q], st, W.h2d_bytes);
       section_raster_kernel<<<(unsigned)std::min<size_t>((N + 255) / 256, 2048), 256, 0, st>>>(sd, p.nx, p.ny, const_cast<cplx *>(r.eps));
     }
     r.mu = nullptr;
@@ -697,6 +706,141 @@ bool batch_refs(const Window &W, const std::vector<int> &ids, std::vector<const 
   return share;
 }
 
+// Derivative pass of one device batch (csrc/derivatives.cuh) on the sorted Ritz vectors: result.dn_dfreq and result.dn_deps of
+// the problems that ask for them.  Reads only; the eigenpairs and fields of the batch are those of a run without it.
+template <typename T, typename C, typename P, typename PC>
+void derivative_pass(b200ms_handle *h, BatchSolver<T, C, P, PC> &S, const std::vector<const ProblemSetup *> &ps, const std::vector<int> &ids,
+                     const Window &W, const b200ms_problem *prob, b200ms_result *res, const std::vector<cd> &nsorted) {
+  const int B = (int)ids.size(), k = S.k, nx = S.nx, ny = S.ny;
+  const size_t N = (size_t)nx * ny;
+  bool any_map = false, any_disp = false;
+  for (int b = 0; b < B; ++b) {
+    const b200ms_problem &p = prob[W.i0 + ids[b]];
+    any_map = any_map || res[W.i0 + ids[b]].dn_deps;
+    any_disp = any_disp || (p.eps ? p.eps_dfreq != nullptr : p.section->deps_table != nullptr);
+  }
+  // host tables: f dc/df = -c kappa / s (kappa / s = Re(l) / l for the stretched length l = s dl k0), metric lengths
+  std::vector<T> dcx((size_t)B * 4 * nx), dcy((size_t)B * 4 * ny);
+  std::vector<cplx> gx((size_t)B * 2 * nx), gy((size_t)B * 2 * ny);
+  const int jz_len = ps[0]->jz_axis >= 0 ? (int)ps[0]->jz_e.size() : 0;
+  std::vector<double> je((size_t)B * jz_len);
+  for (int b = 0; b < B; ++b) {
+    for (int a = 0; a < 2; ++a) {
+      const Axis &A = ps[b]->ax[a];
+      const int n = A.n;
+      std::vector<cd> c;
+      A.coefficients(c);
+      T *dc = (a == 0 ? dcx.data() : dcy.data()) + (size_t)b * 4 * n;
+      cplx *g = (a == 0 ? gx.data() : gy.data()) + (size_t)b * 2 * n;
+      for (int i = 0; i < n; ++i) {
+        const cd rf = A.lf[i].real() / A.lf[i], rb = A.lb[i].real() / A.lb[i];
+        for (int w = 0; w < 4; ++w) dc[(size_t)w * n + i] = from_cd<T>(-c[(size_t)w * n + i] * (w < 2 ? rf : rb));
+        const cd lb = (i == 0 && A.pmc) ? 0.5 * A.lb[i] : A.lb[i];  // PMC wall: half the first dual cell
+        g[i] = mk(A.lf[i].real(), A.lf[i].imag());
+        g[n + i] = mk(lb.real(), lb.imag());
+      }
+    }
+    for (int i = 0; i < jz_len; ++i) je[(size_t)b * jz_len + i] = ps[b]->jz_e[i];
+  }
+  const size_t o_dcx = 0, o_dcy = o_dcx + align256(dcx.size() * sizeof(T)), o_gx = o_dcy + align256(dcy.size() * sizeof(T));
+  const size_t o_gy = o_gx + align256(gx.size() * sizeof(cplx)), o_je = o_gy + align256(gy.size() * sizeof(cplx));
+  const size_t o_part = o_je + align256(std::max<size_t>(1, je.size()) * sizeof(double));
+  const int nch = (int)std::min<size_t>(kDerivChunks, (N + 255) / 256);
+  const size_t o_sum = o_part + align256((size_t)B * k * nch * 3 * sizeof(cplx)), o_scale = o_sum + align256((size_t)B * k * 3 * sizeof(cplx));
+  const size_t o_deps = o_scale + align256((size_t)B * k * sizeof(cplx));
+  size_t o_map = o_deps + (any_disp ? align256((size_t)B * 3 * N * sizeof(cplx)) : 0);
+  size_t sec_bytes = 0;
+  for (int b = 0; b < B; ++b) {
+    const b200ms_problem &p = prob[W.i0 + ids[b]];
+    if (!p.eps && p.section->deps_table) sec_bytes = std::max(sec_bytes, section_device_bytes(*p.section, nx, ny) + align256(9 * N * sizeof(cplx)));
+  }
+  const size_t o_sec = o_map + (any_map ? align256((size_t)B * 3 * N * k * sizeof(cplx)) : 0);
+  h->deriv.reserve(o_sec + sec_bytes + 256);
+  unsigned char *base = h->deriv.p;
+  cudaStream_t st = h->stream;
+  CUDA_CHECK(cudaMemcpyAsync(base + o_dcx, dcx.data(), dcx.size() * sizeof(T), cudaMemcpyHostToDevice, st));
+  CUDA_CHECK(cudaMemcpyAsync(base + o_dcy, dcy.data(), dcy.size() * sizeof(T), cudaMemcpyHostToDevice, st));
+  CUDA_CHECK(cudaMemcpyAsync(base + o_gx, gx.data(), gx.size() * sizeof(cplx), cudaMemcpyHostToDevice, st));
+  CUDA_CHECK(cudaMemcpyAsync(base + o_gy, gy.data(), gy.size() * sizeof(cplx), cudaMemcpyHostToDevice, st));
+  if (jz_len) CUDA_CHECK(cudaMemcpyAsync(base + o_je, je.data(), je.size() * sizeof(double), cudaMemcpyHostToDevice, st));
+  cplx *deps = reinterpret_cast<cplx *>(base + o_deps);
+  if (any_disp) {  // diagonal d eps / df of every problem, [B][3][N]; zero for nondispersive media
+    CUDA_CHECK(cudaMemsetAsync(deps, 0, (size_t)B * 3 * N * sizeof(cplx), st));
+    for (int b = 0; b < B; ++b) {
+      const b200ms_problem &p = prob[W.i0 + ids[b]];
+      const cplx *src = nullptr;
+      if (p.eps && p.eps_dfreq) {
+        src = reinterpret_cast<const cplx *>(p.eps_dfreq);
+      } else if (!p.eps && p.section->deps_table) {  // the medium's rasteriser, fed with the d eps / df table
+        size_t bytes = 0;
+        cplx *full = reinterpret_cast<cplx *>(base + o_sec);
+        SectionDev sd = upload_section(*p.section, p, p.section->deps_table, base + o_sec + align256(9 * N * sizeof(cplx)), st, bytes);
+        section_raster_kernel<<<(unsigned)std::min<size_t>((N + 255) / 256, 2048), 256, 0, st>>>(sd, nx, ny, full);
+        CUDA_CHECK(cudaGetLastError());
+        src = full;
+      }
+      if (!src) continue;
+      for (int a = 0; a < 3; ++a)
+        CUDA_CHECK(cudaMemcpyAsync(deps + ((size_t)b * 3 + a) * N, src + (size_t)(4 * a) * N, N * sizeof(cplx), cudaMemcpyDefault, st));
+      CUDA_CHECK(cudaStreamSynchronize(st));  // the section scratch is reused by the next problem
+    }
+  }
+  DerivArgs<T, C> a;
+  a.nx = nx; a.ny = ny; a.num_modes = k; a.vec = S.ritz_ptr(); a.vstride = S.vstride;
+  a.fields = S.lv[0].fields_true; a.field_bstride = S.lv[0].fbstride; a.cx = S.lv[0].cx_true; a.cy = S.lv[0].cy_true;
+  a.dcx = reinterpret_cast<const T *>(base + o_dcx); a.dcy = reinterpret_cast<const T *>(base + o_dcy);
+  a.gx = reinterpret_cast<const cplx *>(base + o_gx); a.gy = reinterpret_cast<const cplx *>(base + o_gy);
+  a.jz_e = jz_len ? reinterpret_cast<const double *>(base + o_je) : nullptr; a.jz_axis = ps[0]->jz_axis; a.jz_len = jz_len;
+  a.deps = any_disp ? deps : nullptr;
+  a.partial = reinterpret_cast<cplx *>(base + o_part);
+  a.scale = reinterpret_cast<const cplx *>(base + o_scale);
+  a.map = any_map ? reinterpret_cast<cplx *>(base + o_map) : nullptr;
+  cplx *dsum = reinterpret_cast<cplx *>(base + o_sum);
+  {
+    NvtxRange r("b200ms:derivative pass");
+    dim3 g1(nch, B * k);
+    if (S.has_mu) deriv_scan_kernel<T, C, true><<<g1, 256, 0, st>>>(a);
+    else deriv_scan_kernel<T, C, false><<<g1, 256, 0, st>>>(a);
+    deriv_final_kernel<<<(B * k * 3 + 127) / 128, 128, 0, st>>>(a.partial, nch, B * k * 3, dsum);
+    CUDA_CHECK(cudaGetLastError());
+  }
+  std::vector<cplx> sums((size_t)B * k * 3);
+  CUDA_CHECK(cudaMemcpyAsync(sums.data(), dsum, sums.size() * sizeof(cplx), cudaMemcpyDeviceToHost, st));
+  CUDA_CHECK(cudaStreamSynchronize(st));
+  h->stats.launches += 2;
+  // d lambda / df = (w^T (f dA/df) v / f + sum d lambda/d eps . d eps/df) / w^T v;  n = knorm sqrt(-lambda): dn = -knorm d lambda / (2 n)
+  std::vector<cplx> scale((size_t)B * k);
+  for (int b = 0; b < B; ++b) {
+    const b200ms_problem &p = prob[W.i0 + ids[b]];
+    b200ms_result &r = res[W.i0 + ids[b]];
+    for (int q = 0; q < k; ++q) {
+      const cplx *sq = sums.data() + ((size_t)b * k + q) * 3;
+      const cd wv(sq[0].re, sq[0].im), da(sq[1].re, sq[1].im), mat(sq[2].re, sq[2].im);
+      const cd n = nsorted[(size_t)b * k + q];
+      const cd sc = -ps[b]->knorm / (2.0 * n * wv);
+      scale[(size_t)b * k + q] = mk(sc.real(), sc.imag());
+      const cd dn = sc * (da / p.freq + mat);
+      if (r.dn_dfreq) {
+        r.dn_dfreq[2 * q] = dn.real();
+        r.dn_dfreq[2 * q + 1] = dn.imag();
+      }
+    }
+  }
+  if (!any_map) return;
+  CUDA_CHECK(cudaMemcpyAsync(base + o_scale, scale.data(), scale.size() * sizeof(cplx), cudaMemcpyHostToDevice, st));
+  dim3 blk(64, 4), grd((ny + 63) / 64, (nx + 3) / 4, B * k);
+  if (S.has_mu) deriv_map_kernel<T, C, true><<<grd, blk, 0, st>>>(a);
+  else deriv_map_kernel<T, C, false><<<grd, blk, 0, st>>>(a);
+  CUDA_CHECK(cudaGetLastError());
+  h->stats.launches += 1;
+  for (int b = 0; b < B; ++b) {
+    b200ms_result &r = res[W.i0 + ids[b]];
+    if (r.dn_deps)
+      CUDA_CHECK(cudaMemcpyAsync(r.dn_deps, a.map + (size_t)b * 3 * N * k, 3 * N * k * sizeof(cplx), cudaMemcpyDefault, st));
+  }
+  CUDA_CHECK(cudaStreamSynchronize(st));
+}
+
 template <typename T, typename C, typename P, typename PC>
 void solve_group(b200ms_handle *h, const std::vector<int> &ids, const Window &W, const b200ms_problem *prob, b200ms_result *res,
                  unsigned char *out_region, std::vector<FieldCopy> &copies) {
@@ -794,6 +938,9 @@ void solve_group(b200ms_handle *h, const std::vector<int> &ids, const Window &W,
     h->warm_B = B; h->warm_k = k; h->warm_len = S.len; h->warm_tsize = (int)sizeof(T);
     h->warm_valid = true;
   }
+  bool want_deriv = false;
+  for (int b = 0; b < B; ++b) want_deriv = want_deriv || res[W.i0 + ids[b]].dn_dfreq || res[W.i0 + ids[b]].dn_deps;
+  if (want_deriv) derivative_pass(h, S, ps, ids, W, prob, res, nsorted);
   CUDA_CHECK(cudaEventRecord(h->ev1, h->stream));
   CUDA_CHECK(cudaEventSynchronize(h->ev1));
   float ms = 0.f;
@@ -927,10 +1074,17 @@ extern "C" int b200ms_solve_batch(b200ms_handle *h, int nprob, const b200ms_prob
           if (res[i].status == B200MS_OK) res[i].status = s.status;
           res[i].eps_spec = s.eps_spec;
           res[i].is_complex = s.is_complex;
+          std::string err = s.error;
+          if (res[i].status == B200MS_OK && (res[i].dn_dfreq || res[i].dn_deps) && (s.tensorial || s.relative || s.masked)) {
+            res[i].status = B200MS_ERR_UNSUPPORTED;
+            err = s.tensorial ? "mode derivatives: tensorial problems (angled planes, off-diagonal eps) are not supported"
+                  : s.relative ? "mode derivatives: the relative mode solver (basis fields) is not supported"
+                               : "mode derivatives: removed PEC unknowns (mu_cross / split_curl_scaling with PEC cells) are not supported";
+          }
           if (res[i].status != B200MS_OK) {
             if (first_err == B200MS_OK) {
               first_err = res[i].status;
-              h->err = s.error.empty() ? "bad result buffers" : s.error;
+              h->err = err.empty() ? "bad result buffers" : err;
             }
             continue;
           }

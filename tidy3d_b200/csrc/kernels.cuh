@@ -1425,6 +1425,79 @@ struct EpilogueArgs {
   int single;        // write complex64 (precision = "single", solver.py:265-267)
 };
 
+// 1-D difference coefficients [4][n] (f0, f1, b0, bm) of one axis, optionally moved along a direction: c + s dc
+// (zero outside the axis)
+template <typename T>
+struct CoefRows {
+  const T *c, *dc;
+  double s;
+  int n;
+  __device__ __forceinline__ T operator()(int w, int i) const {
+    if (i < 0 || i >= n) return zero_of<T>();
+    T v = ldg(c + (size_t)w * n + i);
+    if (dc) v = v + s * ldg(dc + (size_t)w * n + i);
+    return v;
+  }
+};
+
+// Site arithmetic of the diagonal operator A = P Q at one cell of one problem (solver.py:471-490), shared by the field recovery
+// (epilogue_kernel) and the derivative pass (csrc/derivatives.cuh):
+//   t = imz (Dxf v2 - Dyf v1),  Q v = [q1; q2] = [Dxb t + eyy v2; Dyb t - exx v1],
+//   u = iez (Dxb q2 - Dyb q1) = -iez (Dxb exx v1 + Dyb eyy v2)   (Dxb Dyb = Dyb Dxb),
+//   A v = [Dxf u + myy q2; Dyf u - mxx q1].
+template <typename T, typename C, bool HAS_MU>
+struct DiagSite {
+  const T *v1, *v2;
+  const C *exx, *eyy, *iez, *mxx, *myy, *imz;
+  CoefRows<T> CX, CY;
+  int nx, ny;
+  __device__ __forceinline__ bool in(int ii, int jj) const { return ii >= 0 && ii < nx && jj >= 0 && jj < ny; }
+  __device__ __forceinline__ T V1(int ii, int jj) const { return in(ii, jj) ? ldg(v1 + (size_t)ii * ny + jj) : zero_of<T>(); }
+  __device__ __forceinline__ T V2(int ii, int jj) const { return in(ii, jj) ? ldg(v2 + (size_t)ii * ny + jj) : zero_of<T>(); }
+  __device__ __forceinline__ T TT(int ii, int jj) const {
+    if (!in(ii, jj)) return zero_of<T>();
+    T acc = CX(0, ii) * V2(ii, jj) + CX(1, ii) * V2(ii + 1, jj) - CY(0, jj) * V1(ii, jj) - CY(1, jj) * V1(ii, jj + 1);
+    if (HAS_MU) acc = ldg(imz + (size_t)ii * ny + jj) * acc;
+    return acc;
+  }
+  // Q v at (i, j) (in range); t00 = t(i, j)
+  __device__ __forceinline__ void q(int i, int j, T &q1, T &q2, T &t00) const {
+    const size_t g = (size_t)i * ny + j;
+    const T e1 = V1(i, j), e2 = V2(i, j);
+    const C ex = ldg(exx + g), ey = ldg(eyy + g);
+    t00 = TT(i, j);
+    const T tm0 = TT(i - 1, j), t0m = TT(i, j - 1);
+    q1 = CX(2, i) * t00 + CX(3, i) * tm0 + ey * e2;
+    q2 = CY(2, j) * t00 + CY(3, j) * t0m - ex * e1;
+  }
+  __device__ __forceinline__ T u(int i, int j) const {
+    if (!in(i, j)) return zero_of<T>();
+    const size_t g = (size_t)i * ny + j;
+    const T e1 = V1(i, j), e2 = V2(i, j);
+    const C ex = ldg(exx + g), ey = ldg(eyy + g);
+    T uacc = CX(2, i) * (ex * e1) + CY(2, j) * (ey * e2);
+    if (i > 0) uacc += CX(3, i) * (ldg(exx + g - ny) * V1(i - 1, j));
+    if (j > 0) uacc += CY(3, j) * (ldg(eyy + g - 1) * V2(i, j - 1));
+    return -(ldg(iez + g) * uacc);
+  }
+  // (A v)(i, j) (in range)
+  __device__ __forceinline__ void apply(int i, int j, T &p1, T &p2) const {
+    T q1, q2, t00;
+    q(i, j, q1, q2, t00);
+    const T u0 = u(i, j);
+    p1 = CX(0, i) * u0 + CX(1, i) * u(i + 1, j);
+    p2 = CY(0, j) * u0 + CY(1, j) * u(i, j + 1);
+    if (HAS_MU) {
+      const size_t g = (size_t)i * ny + j;
+      p1 += ldg(myy + g) * q2;
+      p2 -= ldg(mxx + g) * q1;
+    } else {
+      p1 += q2;
+      p2 -= q1;
+    }
+  }
+};
+
 // E = (Ex, Ey, u / (i n)),  H = (-i/eta0) * (q1/(i n), q2/(i n), t)
 // with q1 = Dxb t + eyy v2, q2 = Dyb t - exx v1 (Q v, solver.py:483-489,578-582); the Ez identity
 // iez (Dxb Hy - Dyb Hx) = u/(i n) follows from Dxb Dyb = Dyb Dxb.
@@ -1435,31 +1508,16 @@ __global__ void __launch_bounds__(256) epilogue_kernel(EpilogueArgs<T, C> a) {
   const int j = blockIdx.x * 64 + threadIdx.x, i = blockIdx.y * 4 + threadIdx.y;
   const int m = blockIdx.z % M, b = blockIdx.z / M;
   if (i >= nx || j >= ny) return;
-  const T *v1 = a.vec + (size_t)m * a.vstride + (size_t)b * 2 * N, *v2 = v1 + N;
+  const T *v1 = a.vec + (size_t)m * a.vstride + (size_t)b * 2 * N;
   const C *fb = a.fields + a.field_bstride * b;
-  const C *exx = fb, *eyy = fb + N, *iez = fb + 2 * N, *imz = fb + 5 * N;
-  const T *cx = a.cx + (size_t)b * 4 * nx, *cy = a.cy + (size_t)b * 4 * ny;
-  const T z = zero_of<T>();
-  auto V1 = [&](int ii, int jj) { return (ii >= 0 && ii < nx && jj >= 0 && jj < ny) ? ldg(v1 + (size_t)ii * ny + jj) : z; };
-  auto V2 = [&](int ii, int jj) { return (ii >= 0 && ii < nx && jj >= 0 && jj < ny) ? ldg(v2 + (size_t)ii * ny + jj) : z; };
-  auto CX = [&](int w, int ii) { return (ii >= 0 && ii < nx) ? ldg(cx + (size_t)w * nx + ii) : z; };
-  auto CY = [&](int w, int jj) { return (jj >= 0 && jj < ny) ? ldg(cy + (size_t)w * ny + jj) : z; };
-  auto TT = [&](int ii, int jj) {
-    if (ii < 0 || jj < 0 || ii >= nx || jj >= ny) return z;
-    T acc = CX(0, ii) * V2(ii, jj) + CX(1, ii) * V2(ii + 1, jj) - CY(0, jj) * V1(ii, jj) - CY(1, jj) * V1(ii, jj + 1);
-    if (HAS_MU) acc = ldg(imz + (size_t)ii * ny + jj) * acc;
-    return acc;
-  };
+  const DiagSite<T, C, HAS_MU> S{v1, v1 + N, fb, fb + N, fb + 2 * N, fb + 3 * N, fb + 4 * N, fb + 5 * N,
+                                 CoefRows<T>{a.cx + (size_t)b * 4 * nx, nullptr, 0.0, nx}, CoefRows<T>{a.cy + (size_t)b * 4 * ny, nullptr, 0.0, ny},
+                                 nx, ny};
   const size_t g = (size_t)i * ny + j;
-  const T e1 = V1(i, j), e2 = V2(i, j);
-  const C ex = ldg(exx + g), ey = ldg(eyy + g);
-  const T t00 = TT(i, j), tm0 = TT(i - 1, j), t0m = TT(i, j - 1);
-  const T q1 = CX(2, i) * t00 + CX(3, i) * tm0 + ey * e2;
-  const T q2 = CY(2, j) * t00 + CY(3, j) * t0m - ex * e1;
-  T uacc = CX(2, i) * (ex * e1) + CY(2, j) * (ey * e2);
-  if (i > 0) uacc += CX(3, i) * (ldg(exx + g - ny) * V1(i - 1, j));
-  if (j > 0) uacc += CY(3, j) * (ldg(eyy + g - 1) * V2(i, j - 1));
-  const T u = -(ldg(iez + g) * uacc);
+  T q1, q2, t00;
+  S.q(i, j, q1, q2, t00);
+  const T e1 = S.V1(i, j), e2 = S.V2(i, j);
+  const T u = S.u(i, j);
   const cplx nc = a.ncomplex[(size_t)b * M + m];
   const cplx inv_in = recip(mk(-nc.im, nc.re));  // 1 / (i n)
   const cplx hs = mk(0.0, -a.h_scale);           // -i / eta0

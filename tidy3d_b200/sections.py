@@ -82,6 +82,14 @@ class Medium:
             return e.astype(complex)
         raise ValueError("Medium.eps must be a scalar, 3 numbers or a 3x3 tensor")
 
+    def dtensor_dfreq(self, freq: float) -> np.ndarray:
+        """d eps / df (1/Hz) of the 3x3 tensor: zero for a constant medium, a central difference of ``eps(f)`` with a relative
+        step of 1e-4 (error O(step^2) for a smooth model) for a dispersive one; the material term of the mode derivatives."""
+        if not callable(self.eps):
+            return np.zeros((3, 3), dtype=complex)
+        h = 1e-4 * freq
+        return (self.tensor(freq + h) - self.tensor(freq - h)) / (2 * h)
+
 
 def site_medium_from_masks(shape: Tuple[int, int], masks: Sequence[Tuple[np.ndarray, int]]) -> np.ndarray:
     """(3, Nx, Ny) uint16 site map from per-structure inside-masks, drawn in structure order like epsilon_on_grid
@@ -143,9 +151,10 @@ class Section:
             raise ValueError("Mismatch between 'coords' and 'site_medium' shapes.")
         return sm
 
-    def pack(self, freq: float, shape: Optional[Tuple[int, int]] = None):
+    def pack(self, freq: float, shape: Optional[Tuple[int, int]] = None, dispersion: bool = False):
         """ctypes ``b200ms_section`` for one frequency plus the arrays it points to (kept alive by the caller).  ``shape`` =
-        (Nx, Ny) of the plane, needed to check ``site_medium``."""
+        (Nx, Ny) of the plane, needed to check ``site_medium``.  ``dispersion``: also pass every medium's d eps / df
+        (``deps_table``), the material term of the mode derivatives."""
         media, ids = self._media()
         n = len(self.structures)
         rects = np.zeros((n, 4), dtype=np.float64)
@@ -188,4 +197,8 @@ class Section:
             st.poly_xy = pxy.ctypes.data_as(_cabi._dp)
         if site is not None:
             st.site_medium = site.ctypes.data_as(C.POINTER(C.c_ushort))
-        return st, (rects, med, table, kinds, pstart, pxy, site)
+        dtable = None
+        if dispersion and any(callable(m.eps) for m in media):
+            dtable = np.ascontiguousarray([m.dtensor_dfreq(freq).ravel() for m in media], dtype=np.complex128)
+            st.deps_table = dtable.view(np.float64).ctypes.data_as(_cabi._dp)
+        return st, (rects, med, table, kinds, pstart, pxy, site, dtable)

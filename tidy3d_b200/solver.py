@@ -78,7 +78,7 @@ def _undo_split_curl(fields, split):
 
 def compute_modes_batch(
     problems: Sequence[dict], device: int = -1, want_fields: bool = True, return_info: bool = False, handle=None,
-    fields_ptrs=None, post: Optional[Sequence[str]] = None,
+    fields_ptrs=None, post: Optional[Sequence[str]] = None, derivatives: Optional[Sequence[str]] = None,
 ):
     """Solve many independent mode problems in one device call.
 
@@ -98,11 +98,22 @@ def compute_modes_batch(
     finite-grid correction factors of ``ModeSolver._grid_correction`` (mode_solver.py:847-904), like the reference's; and
     ``plane_bounds=(xmin, xmax, ymin, ymax)`` (``plugin.plane_bounds_of``): the extent of a finite mode plane, to which the
     integration weights are truncated like the reference's ``_diff_area`` (monitor_data.py:437-455).
+
+    ``derivatives``: first-order derivatives of every mode from its own solve (left eigenvector, no extra solves; diagonal
+    problems only, else ``NotImplementedError``).  ``"freq"`` adds ``dn_dfreq`` (d(n_eff + i k_eff)/df, 1/Hz) and ``n_group``
+    (n_eff + f Re(dn/df), what ``ModeData._group_index_post_process`` approximates from three solves) to the info dict;
+    ``"eps"`` adds ``dn_deps`` (3, Nx, Ny, M): d(n_eff + i k_eff) / d eps_{xx,yy,zz} of ``eps_cross`` at every Yee site (PML stretch
+    held fixed).  Material dispersion enters ``dn_dfreq`` through a problem's ``eps_dfreq=`` (d eps_cross / df) or, for a
+    ``section``, through the media whose ``eps`` is a callable.  ``n_complex`` and the fields do not change.
     """
     post = tuple(post or ())
     unknown = set(post) - {"gauge", "normalize", "flux", "overlaps"}
     if unknown:
         raise ValueError(f"unknown post-processing step(s): {sorted(unknown)}")
+    derivatives = tuple(derivatives or ())
+    unknown = set(derivatives) - {"freq", "eps"}
+    if unknown:
+        raise ValueError(f"unknown derivative(s): {sorted(unknown)}")
     post_flags = (1 if "gauge" in post else 0) | (2 if "normalize" in post else 0)
     packed, cache = [], {}
     for p in problems:
@@ -127,6 +138,7 @@ def compute_modes_batch(
             mu_cross=p.get("mu_cross"), target_override=target_override,
             incidence=(split is not None or p.get("mu_cross") is not None),  # solver.py:93
             post=post_flags, grid_correction=p.get("grid_correction"), plane_bounds=p.get("plane_bounds"),
+            eps_dfreq=p.get("eps_dfreq"), derivatives="freq" in derivatives,
         )  # fmt: skip
         if split is None and section is None:
             cache[key] = pk.eps
@@ -139,9 +151,11 @@ def compute_modes_batch(
         packed.append(pk)
     h = handle or get_handle(device)  # after input validation: argument errors do not need a GPU
     with h.lock:
+        dkw = dict(want_dfreq="freq" in derivatives, want_deps="eps" in derivatives) if derivatives else {}
         rc, fields, ncs, results = h.solve_batch(packed, want_fields, fields_ptrs, want_flux=("flux" in post or "normalize" in post),
-                                                 want_overlaps="overlaps" in post)
+                                                 want_overlaps="overlaps" in post, **dkw)
         flux_out, te_out, ov_out = h.last_flux, h.last_te, h.last_overlaps
+        dfreq_out, deps_out = (h.last_dn_dfreq, h.last_dn_deps) if derivatives else ([], [])
         err = h.last_error() if rc != _cabi.OK else ""
     if rc != _cabi.OK:
         bad = [i for i in range(len(packed)) if results[i].status != _cabi.OK]
@@ -163,6 +177,11 @@ def compute_modes_batch(
             infos[-1]["te_fraction"] = te_out[i]
         if ov_out:
             infos[-1]["overlap_prev"] = ov_out[i]
+        if dfreq_out:
+            infos[-1]["dn_dfreq"] = dfreq_out[i]
+            infos[-1]["n_group"] = ncs[i].real + float(packed[i].struct.freq) * dfreq_out[i].real
+        if deps_out:
+            infos[-1]["dn_deps"] = deps_out[i]
     return (out, infos) if return_info else out
 
 

@@ -1,0 +1,103 @@
+"""Group index three ways on the headline workload (Si strip 512x512, 4 modes), alternated in one process:
+  plain   -- one solve per frequency, no derivatives;
+  analytic -- one solve per frequency with derivatives=("freq",) (n_group from the left eigenvector);
+  fd3     -- three solves per frequency at f(1 -/+ step) and f, n_group by plugin.group_index (the reference's path).
+Prints one JSON line: solves/s, frequencies-with-group-index/s, the device time the derivative pass adds per problem and the
+pass's algorithmic bytes against the 3.35 TB/s HBM3 data-sheet figure, with the card name and power limit read in the same run.
+
+    python tools/bench_derivatives.py [--nf 64] [--rounds 2] [--n 512] [--out results/bench_derivatives.json]
+"""
+import argparse
+import json
+import os
+import subprocess
+import sys
+import time
+
+import numpy as np
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+
+
+def card():
+    try:
+        q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True, timeout=30)
+        return q.stdout.strip()
+    except Exception as e:  # noqa: BLE001
+        return f"unknown ({e})"
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--nf", type=int, default=64)
+    ap.add_argument("--rounds", type=int, default=2)
+    ap.add_argument("--n", type=int, default=512)
+    ap.add_argument("--step", type=float, default=1e-3)
+    ap.add_argument("--out", default=None)
+    a = ap.parse_args()
+    import torch
+
+    if not torch.cuda.is_available():
+        raise SystemExit("no CUDA device: this benchmark measures the GPU only")
+    from tidy3d_b200 import plugin
+    from tidy3d_b200 import workloads as W
+    from tidy3d_b200.solver import compute_modes_batch, get_handle
+
+    wl = W.headline(nf=a.nf, n=a.n)
+    eps = np.ascontiguousarray(np.stack(wl.eps_cross))
+    h = get_handle()
+
+    def probs(freqs):
+        return [dict(eps_cross=eps, coords=wl.coords, freq=float(f), mode_spec=wl.mode_spec) for f in freqs]
+
+    f3 = np.outer(wl.freqs, (1 - a.step, 1, 1 + a.step)).ravel()
+    arms = {
+        "plain": lambda: compute_modes_batch(probs(wl.freqs), handle=h, want_fields=False, return_info=True),
+        "analytic": lambda: compute_modes_batch(probs(wl.freqs), handle=h, want_fields=False, return_info=True, derivatives=("freq",)),
+        "fd3": lambda: compute_modes_batch(probs(f3), handle=h, want_fields=False, return_info=True),
+    }
+    for fn in arms.values():  # warm-up of every shape
+        fn()
+    t = {k: [] for k in arms}
+    dev = {k: [] for k in arms}
+    ng = {}
+    for _ in range(a.rounds):
+        for k, fn in arms.items():
+            torch.cuda.synchronize()
+            t0 = time.perf_counter()
+            out, infos = fn()
+            torch.cuda.synchronize()
+            t[k].append(time.perf_counter() - t0)
+            dev[k].append(h.last_stats()["device_ms"])
+            if k == "analytic":
+                ng["analytic"] = np.array([i["n_group"] for i in infos])
+            if k == "fd3":
+                ng["fd3"] = plugin.group_index(np.array([o[1] for o in out]), f3, a.step)[2]
+    nsolve = {"plain": a.nf, "analytic": a.nf, "fd3": 3 * a.nf}
+    N, M = a.n * a.n, wl.mode_spec.num_modes
+    # one derivative pass reads, per (problem, mode), the real fp64 Ritz vector (2N x 8 B) and the three coefficient fields
+    # (exx, eyy, 1/ezz: 3N x 8 B; shared by the sweep, counted once per mode pass as they are re-read)
+    bytes_pass = a.nf * M * (2 * N * 8 + 3 * N * 8)
+    extra_ms = (np.median(dev["analytic"]) - np.median(dev["plain"]))
+    res = dict(
+        card=card(), workload=f"headline {a.n}x{a.n}, {M} modes, {a.nf} frequencies", rounds=a.rounds,
+        solves_per_s={k: nsolve[k] / float(np.median(v)) for k, v in t.items()},
+        freqs_with_group_index_per_s={"analytic": a.nf / float(np.median(t["analytic"])), "fd3": a.nf / float(np.median(t["fd3"]))},
+        device_ms_median={k: float(np.median(v)) for k, v in dev.items()},
+        derivative_pass_device_ms_per_problem=float(extra_ms / a.nf),
+        derivative_pass_bytes=bytes_pass,
+        derivative_pass_bw_TBps=float(bytes_pass / max(extra_ms, 1e-9) / 1e9),
+        hbm_datasheet_TBps=3.35,
+        n_group_max_abs_diff_analytic_vs_fd3=float(np.abs(ng["analytic"] - ng["fd3"]).max()),
+    )  # fmt: skip
+    line = json.dumps(res)
+    print(line)
+    if a.out:
+        os.makedirs(os.path.dirname(a.out) or ".", exist_ok=True)
+        with open(a.out, "w") as f:
+            f.write(line + "\n")
+
+
+if __name__ == "__main__":
+    main()
