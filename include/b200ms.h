@@ -29,7 +29,7 @@
 extern "C" {
 #endif
 
-#define B200MS_VERSION 205
+#define B200MS_VERSION 206
 
 /* return codes */
 enum {
@@ -93,6 +93,9 @@ typedef struct {
   const double *deps_table; /* NULL (nondispersive media), or nmedia x 9 complex128 (re,im): d eps / df (1/Hz) of each medium at this
                               problem's frequency, rasterised like eps_table; only the material term of result.dn_dfreq reads it
                               (diagonal components) */
+  /* ---- since version 206 ---- */
+  const double *d2eps_table; /* NULL, or nmedia x 9 complex128 (re,im): d^2 eps / df^2 (1/Hz^2) of each medium at this problem's
+                              frequency, rasterised like eps_table; only result.d2n_dfreq2 reads it (diagonal components) */
 } b200ms_section;
 
 /* One eigenproblem == one compute_modes call (one plane, one frequency). */
@@ -140,6 +143,8 @@ typedef struct {
                             points clipped to monitor.bounds).  Only the post-processing results depend on it */
   const double *eps_dfreq; /* since version 205.  NULL (nondispersive medium), or d eps_cross / df (1/Hz) in the layout of `eps`; only the
                             diagonal components are read, and only by the material term of result.dn_dfreq */
+  const double *eps_d2freq; /* since version 206.  NULL, or d^2 eps_cross / df^2 (1/Hz^2) in the layout of `eps`; only the diagonal
+                            components are read, and only by result.d2n_dfreq2 */
 } b200ms_problem;
 
 typedef struct {
@@ -180,6 +185,16 @@ typedef struct {
   double *dn_deps;       /* NULL, or caller-allocated 3*nx*ny*num_modes complex128 (re,im), [xx|yy|zz][ix][iy][mode]: d(n_eff + i k_eff)
                             / d eps_aa of the caller's eps_cross at the Ex / Ey / Ez site of each cell (PML stretch held fixed; 0 at
                             PEC-valued cells); HOST or DEVICE memory like `fields` */
+  /* ---- since version 206: second frequency derivative of each mode (group-velocity dispersion).  One correction solve
+     (A - lambda) x = -Pi (dA/df - dlambda/df) v per mode, Pi = I - v w^T / (w^T v), then
+     d2lambda/df2 = [w^T (d2A/df2) v + 2 w^T (dA/df - dlambda/df) x] / (w^T v) (see DESIGN.md §4).  Same scope as dn_dfreq;
+     n_complex, the fields, dn_dfreq and dn_deps do not change when it is asked for ---- */
+  double *d2n_dfreq2;    /* NULL, or caller-allocated num_modes complex128 (re,im): d^2(n_eff + i k_eff)/df^2 (1/Hz^2), including the
+                            material dispersion of problem.eps_dfreq / eps_d2freq (section: deps_table / d2eps_table).  NaN for a mode
+                            whose correction solve stopped above 100 x inner_tol.  Dispersion (ps/(nm km)):
+                            D = -1e18 f^2 (2 Re dn/df + f Re d2n/df2) / c0^2, c0 in um/s */
+  double *d2n_residual;  /* NULL, or caller-allocated num_modes doubles: final relative residual of each mode's correction solve
+                            (needs d2n_dfreq2) */
 } b200ms_result;
 
 /* Tunables (all have defaults; see DESIGN.md). */

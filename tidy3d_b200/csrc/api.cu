@@ -62,6 +62,7 @@ struct b200ms_handle {
   DevBuf refs;        // MediumRef array of the batch being built
   DevBuf post;        // interpolation tables / partials / results of the on-device post-processing
   DevBuf deriv;       // tables, partial sums, dispersion input and d n / d eps map of the derivative pass
+  DevBuf disp;        // tables, material directions and partial sums of the dispersion pass
   DevBuf warm;        // sorted Ritz vectors of the previous device batch of this call ([k][B][len]): warm start of the next one
   int warm_B = 0, warm_k = 0, warm_tsize = 0;
   size_t warm_len = 0;
@@ -156,6 +157,7 @@ extern "C" int b200ms_destroy(b200ms_handle *h) {
   h->post.release();
   h->warm.release();
   h->deriv.release();
+  h->disp.release();
   if (h->io_stream) cudaStreamDestroy(h->io_stream);
   if (h->dl_stream) cudaStreamDestroy(h->dl_stream);
   if (h->flush_buf) cudaFree(h->flush_buf);
@@ -706,11 +708,54 @@ bool batch_refs(const Window &W, const std::vector<int> &ids, std::vector<const 
   return share;
 }
 
+// The diagonal (xx, yy, zz) of a per-problem input in the layout of `eps` -- the caller's array `arr(p)`, or for a section the
+// rasteriser fed with the per-medium table `tab(sec)` -- into dst [B][3][N], zero where a problem has neither.  `scratch` holds
+// one rasterised section (9 N complex values, then the section upload); the stream is synchronised after every problem.
+template <typename Arr, typename Tab>
+void gather_diag(b200ms_handle *h, const std::vector<int> &ids, const Window &W, const b200ms_problem *prob, int nx, int ny, Arr arr,
+                 Tab tab, cplx *dst, unsigned char *scratch) {
+  const int B = (int)ids.size();
+  const size_t N = (size_t)nx * ny;
+  cudaStream_t st = h->stream;
+  CUDA_CHECK(cudaMemsetAsync(dst, 0, (size_t)B * 3 * N * sizeof(cplx), st));
+  for (int b = 0; b < B; ++b) {
+    const b200ms_problem &p = prob[W.i0 + ids[b]];
+    const cplx *src = nullptr;
+    if (p.eps && arr(p)) {
+      src = reinterpret_cast<const cplx *>(arr(p));
+    } else if (!p.eps && tab(*p.section)) {  // the medium's rasteriser, fed with the derivative table
+      size_t bytes = 0;
+      cplx *full = reinterpret_cast<cplx *>(scratch);
+      SectionDev sd = upload_section(*p.section, p, tab(*p.section), scratch + align256(9 * N * sizeof(cplx)), st, bytes);
+      section_raster_kernel<<<(unsigned)std::min<size_t>((N + 255) / 256, 2048), 256, 0, st>>>(sd, nx, ny, full);
+      CUDA_CHECK(cudaGetLastError());
+      src = full;
+    }
+    if (!src) continue;
+    for (int a = 0; a < 3; ++a)
+      CUDA_CHECK(cudaMemcpyAsync(dst + ((size_t)b * 3 + a) * N, src + (size_t)(4 * a) * N, N * sizeof(cplx), cudaMemcpyDefault, st));
+    CUDA_CHECK(cudaStreamSynchronize(st));  // the section scratch is reused by the next problem
+  }
+}
+
+// bytes of gather_diag's scratch for the sections of a batch that carry the table `tab`
+template <typename Tab>
+size_t gather_scratch_bytes(const std::vector<int> &ids, const Window &W, const b200ms_problem *prob, int nx, int ny, Tab tab) {
+  size_t bytes = 0;
+  for (int id : ids) {
+    const b200ms_problem &p = prob[W.i0 + id];
+    if (!p.eps && tab(*p.section))
+      bytes = std::max(bytes, section_device_bytes(*p.section, nx, ny) + align256(9 * (size_t)nx * ny * sizeof(cplx)));
+  }
+  return bytes;
+}
+
 // Derivative pass of one device batch (csrc/derivatives.cuh) on the sorted Ritz vectors: result.dn_dfreq and result.dn_deps of
-// the problems that ask for them.  Reads only; the eigenpairs and fields of the batch are those of a run without it.
+// the problems that ask for them.  Reads only; the eigenpairs and fields of the batch are those of a run without it.  `out`
+// receives the pass's device tables (valid until h->deriv is reserved again) for the dispersion pass.
 template <typename T, typename C, typename P, typename PC>
 void derivative_pass(b200ms_handle *h, BatchSolver<T, C, P, PC> &S, const std::vector<const ProblemSetup *> &ps, const std::vector<int> &ids,
-                     const Window &W, const b200ms_problem *prob, b200ms_result *res, const std::vector<cd> &nsorted) {
+                     const Window &W, const b200ms_problem *prob, b200ms_result *res, const std::vector<cd> &nsorted, DerivArgs<T, C> &out) {
   const int B = (int)ids.size(), k = S.k, nx = S.nx, ny = S.ny;
   const size_t N = (size_t)nx * ny;
   bool any_map = false, any_disp = false;
@@ -749,11 +794,9 @@ void derivative_pass(b200ms_handle *h, BatchSolver<T, C, P, PC> &S, const std::v
   const size_t o_sum = o_part + align256((size_t)B * k * nch * 3 * sizeof(cplx)), o_scale = o_sum + align256((size_t)B * k * 3 * sizeof(cplx));
   const size_t o_deps = o_scale + align256((size_t)B * k * sizeof(cplx));
   size_t o_map = o_deps + (any_disp ? align256((size_t)B * 3 * N * sizeof(cplx)) : 0);
-  size_t sec_bytes = 0;
-  for (int b = 0; b < B; ++b) {
-    const b200ms_problem &p = prob[W.i0 + ids[b]];
-    if (!p.eps && p.section->deps_table) sec_bytes = std::max(sec_bytes, section_device_bytes(*p.section, nx, ny) + align256(9 * N * sizeof(cplx)));
-  }
+  auto arr1 = [](const b200ms_problem &p) { return p.eps_dfreq; };
+  auto tab1 = [](const b200ms_section &sec) { return sec.deps_table; };
+  const size_t sec_bytes = gather_scratch_bytes(ids, W, prob, nx, ny, tab1);
   const size_t o_sec = o_map + (any_map ? align256((size_t)B * 3 * N * k * sizeof(cplx)) : 0);
   h->deriv.reserve(o_sec + sec_bytes + 256);
   unsigned char *base = h->deriv.p;
@@ -764,27 +807,7 @@ void derivative_pass(b200ms_handle *h, BatchSolver<T, C, P, PC> &S, const std::v
   CUDA_CHECK(cudaMemcpyAsync(base + o_gy, gy.data(), gy.size() * sizeof(cplx), cudaMemcpyHostToDevice, st));
   if (jz_len) CUDA_CHECK(cudaMemcpyAsync(base + o_je, je.data(), je.size() * sizeof(double), cudaMemcpyHostToDevice, st));
   cplx *deps = reinterpret_cast<cplx *>(base + o_deps);
-  if (any_disp) {  // diagonal d eps / df of every problem, [B][3][N]; zero for nondispersive media
-    CUDA_CHECK(cudaMemsetAsync(deps, 0, (size_t)B * 3 * N * sizeof(cplx), st));
-    for (int b = 0; b < B; ++b) {
-      const b200ms_problem &p = prob[W.i0 + ids[b]];
-      const cplx *src = nullptr;
-      if (p.eps && p.eps_dfreq) {
-        src = reinterpret_cast<const cplx *>(p.eps_dfreq);
-      } else if (!p.eps && p.section->deps_table) {  // the medium's rasteriser, fed with the d eps / df table
-        size_t bytes = 0;
-        cplx *full = reinterpret_cast<cplx *>(base + o_sec);
-        SectionDev sd = upload_section(*p.section, p, p.section->deps_table, base + o_sec + align256(9 * N * sizeof(cplx)), st, bytes);
-        section_raster_kernel<<<(unsigned)std::min<size_t>((N + 255) / 256, 2048), 256, 0, st>>>(sd, nx, ny, full);
-        CUDA_CHECK(cudaGetLastError());
-        src = full;
-      }
-      if (!src) continue;
-      for (int a = 0; a < 3; ++a)
-        CUDA_CHECK(cudaMemcpyAsync(deps + ((size_t)b * 3 + a) * N, src + (size_t)(4 * a) * N, N * sizeof(cplx), cudaMemcpyDefault, st));
-      CUDA_CHECK(cudaStreamSynchronize(st));  // the section scratch is reused by the next problem
-    }
-  }
+  if (any_disp) gather_diag(h, ids, W, prob, nx, ny, arr1, tab1, deps, base + o_sec);  // diagonal d eps / df, [B][3][N]
   DerivArgs<T, C> a;
   a.nx = nx; a.ny = ny; a.num_modes = k; a.vec = S.ritz_ptr(); a.vstride = S.vstride;
   a.fields = S.lv[0].fields_true; a.field_bstride = S.lv[0].fbstride; a.cx = S.lv[0].cx_true; a.cy = S.lv[0].cy_true;
@@ -796,6 +819,7 @@ void derivative_pass(b200ms_handle *h, BatchSolver<T, C, P, PC> &S, const std::v
   a.scale = reinterpret_cast<const cplx *>(base + o_scale);
   a.map = any_map ? reinterpret_cast<cplx *>(base + o_map) : nullptr;
   cplx *dsum = reinterpret_cast<cplx *>(base + o_sum);
+  out = a;
   {
     NvtxRange r("b200ms:derivative pass");
     dim3 g1(nch, B * k);
@@ -839,6 +863,139 @@ void derivative_pass(b200ms_handle *h, BatchSolver<T, C, P, PC> &S, const std::v
       CUDA_CHECK(cudaMemcpyAsync(r.dn_deps, a.map + (size_t)b * 3 * N * k, 3 * N * k * sizeof(cplx), cudaMemcpyDefault, st));
   }
   CUDA_CHECK(cudaStreamSynchronize(st));
+}
+
+
+// Dispersion pass of one device batch (csrc/derivatives.cuh), after derivative_pass (whose device tables `da` it reads):
+// result.d2n_dfreq2 and result.d2n_residual of the problems that ask for them.  Per mode slot q: the projected right-hand side
+// r = -Pi A'v, one correction solve (A - lambda_q) x = r by the eigen-solve's own inner solver (Krylov shift lambda_q of every
+// problem; the multigrid stays built for sigma) and a scan for w^T A'x.  It writes its own buffers, the first two slots of the
+// outer Krylov basis and the inner solver's scratch -- nothing the fields, the post-processing or the warm start read.
+template <typename T, typename C, typename P, typename PC>
+void dispersion_pass(b200ms_handle *h, BatchSolver<T, C, P, PC> &S, const std::vector<const ProblemSetup *> &ps, const std::vector<int> &ids,
+                     const Window &W, const b200ms_problem *prob, b200ms_result *res, const std::vector<cd> &nsorted,
+                     const std::vector<cd> &lam, const DerivArgs<T, C> &da) {
+  const int B = (int)ids.size(), k = S.k, nx = S.nx, ny = S.ny;
+  const size_t N = (size_t)nx * ny;
+  std::vector<char> skip(B);
+  bool any_mat = false;
+  for (int b = 0; b < B; ++b) {
+    const b200ms_problem &p = prob[W.i0 + ids[b]];
+    skip[b] = res[W.i0 + ids[b]].d2n_dfreq2 ? 0 : 1;
+    any_mat = any_mat || (p.eps ? (p.eps_dfreq || p.eps_d2freq) : (p.section->deps_table || p.section->d2eps_table));
+  }
+  // host tables: f^2 d^2c/df^2 = 2 (f dc/df)^2 / c = 2 c (kappa / s)^2, frequencies
+  std::vector<T> c2x((size_t)B * 4 * nx), c2y((size_t)B * 4 * ny);
+  std::vector<double> freq(B);
+  for (int b = 0; b < B; ++b) {
+    freq[b] = prob[W.i0 + ids[b]].freq;
+    for (int a = 0; a < 2; ++a) {
+      const Axis &A = ps[b]->ax[a];
+      const int n = A.n;
+      std::vector<cd> c;
+      A.coefficients(c);
+      T *c2 = (a == 0 ? c2x.data() : c2y.data()) + (size_t)b * 4 * n;
+      for (int i = 0; i < n; ++i) {
+        const cd rf = A.lf[i].real() / A.lf[i], rb = A.lb[i].real() / A.lb[i];
+        for (int w = 0; w < 4; ++w) {
+          const cd r = w < 2 ? rf : rb;
+          c2[(size_t)w * n + i] = from_cd<T>(2.0 * c[(size_t)w * n + i] * r * r);
+        }
+      }
+    }
+  }
+  auto arr1 = [](const b200ms_problem &p) { return p.eps_dfreq; };
+  auto tab1 = [](const b200ms_section &sec) { return sec.deps_table; };
+  auto arr2 = [](const b200ms_problem &p) { return p.eps_d2freq; };
+  auto tab2 = [](const b200ms_section &sec) { return sec.d2eps_table; };
+  const int nch = (int)std::min<size_t>(kDerivChunks, (N + 255) / 256);
+  const size_t o_c2x = 0, o_c2y = align256(c2x.size() * sizeof(T)), o_f = o_c2y + align256(c2y.size() * sizeof(T));
+  const size_t o_part = o_f + align256(B * sizeof(double)), o_sum = o_part + align256((size_t)B * nch * 3 * sizeof(cplx));
+  const size_t o_beta = o_sum + align256((size_t)B * 3 * sizeof(cplx)), o_p1 = o_beta + align256(B * sizeof(cplx));
+  const size_t pbytes = any_mat ? align256((size_t)B * 3 * N * sizeof(cplx)) : 0, o_p2 = o_p1 + pbytes, o_sec = o_p2 + pbytes;
+  const size_t sec_bytes = any_mat ? std::max(gather_scratch_bytes(ids, W, prob, nx, ny, tab1), gather_scratch_bytes(ids, W, prob, nx, ny, tab2)) : 0;
+  h->disp.reserve(o_sec + sec_bytes + 256);
+  unsigned char *base = h->disp.p;
+  cudaStream_t st = h->stream;
+  CUDA_CHECK(cudaMemcpyAsync(base + o_c2x, c2x.data(), c2x.size() * sizeof(T), cudaMemcpyHostToDevice, st));
+  CUDA_CHECK(cudaMemcpyAsync(base + o_c2y, c2y.data(), c2y.size() * sizeof(T), cudaMemcpyHostToDevice, st));
+  CUDA_CHECK(cudaMemcpyAsync(base + o_f, freq.data(), B * sizeof(double), cudaMemcpyHostToDevice, st));
+  DispArgs<T, C> a;
+  a.d = da;
+  a.c2x = reinterpret_cast<const T *>(base + o_c2x);
+  a.c2y = reinterpret_cast<const T *>(base + o_c2y);
+  a.p1 = a.p2 = nullptr;
+  if (any_mat) {  // f dp/df and f^2 d^2p/df^2 of the solver-frame (exx, eyy, 1/ezz)
+    cplx *p1 = reinterpret_cast<cplx *>(base + o_p1), *p2 = reinterpret_cast<cplx *>(base + o_p2);
+    gather_diag(h, ids, W, prob, nx, ny, arr1, tab1, p1, base + o_sec);
+    gather_diag(h, ids, W, prob, nx, ny, arr2, tab2, p2, base + o_sec);
+    disp_fields_kernel<C><<<(unsigned)std::min<size_t>(((size_t)B * N + 255) / 256, 4096), 256, 0, st>>>(
+        nx, ny, B, da.fields, da.field_bstride, da.jz_e, da.jz_axis, da.jz_len, reinterpret_cast<const double *>(base + o_f), p1, p2);
+    CUDA_CHECK(cudaGetLastError());
+    h->stats.launches += 1;
+    a.p1 = p1;
+    a.p2 = p2;
+  }
+  a.partial = reinterpret_cast<cplx *>(base + o_part);
+  cplx *dsum = reinterpret_cast<cplx *>(base + o_sum), *dbeta = reinterpret_cast<cplx *>(base + o_beta);
+  a.beta = dbeta;
+  T *r = S.basis0(), *x = S.basis0() + S.vstride;
+  a.r = r;
+  a.x = x;
+  auto scan = [&](int phase, std::vector<cplx> &sums) {
+    const dim3 g(phase == 1 ? (unsigned)std::min<size_t>((N + 255) / 256, 1024) : (unsigned)nch, B);
+    if (S.has_mu) disp_scan_kernel<T, C, true><<<g, 256, 0, st>>>(a, phase);
+    else disp_scan_kernel<T, C, false><<<g, 256, 0, st>>>(a, phase);
+    h->stats.launches += 1;
+    if (phase == 1) return;
+    deriv_final_kernel<<<(B * 3 + 127) / 128, 128, 0, st>>>(a.partial, nch, B * 3, dsum);
+    CUDA_CHECK(cudaGetLastError());
+    h->stats.launches += 1;
+    sums.resize((size_t)B * 3);
+    CUDA_CHECK(cudaMemcpyAsync(sums.data(), dsum, sums.size() * sizeof(cplx), cudaMemcpyDeviceToHost, st));
+    CUDA_CHECK(cudaStreamSynchronize(st));
+  };
+  const double tol = h->opt.inner_tol;
+  NvtxRange nr("b200ms:dispersion pass");
+  for (int q = 0; q < k; ++q) {
+    a.q = q;
+    std::vector<cplx> sv, sx;
+    scan(0, sv);  // w^T v, w^T A'v, w^T A''v
+    std::vector<cplx> beta(B);
+    std::vector<cd> shift(B);
+    for (int b = 0; b < B; ++b) {
+      const cplx *s = sv.data() + (size_t)b * 3;
+      const cd wv(s[0].re, s[0].im), w1(s[1].re, s[1].im);
+      const cd be = std::abs(wv) > 0 ? w1 / wv : cd(0, 0);
+      beta[b] = mk(be.real(), be.imag());
+      shift[b] = lam[(size_t)b * k + q];
+    }
+    CUDA_CHECK(cudaMemcpyAsync(dbeta, beta.data(), B * sizeof(cplx), cudaMemcpyHostToDevice, st));
+    scan(1, sx);  // r = -(A'v - beta v)
+    S.set_sigma(shift);
+    int iters = 0;
+    std::vector<double> resv;
+    S.solve_op(r, x, iters, &skip, nullptr, &resv);
+    scan(2, sx);  // w^T x, w^T A'x
+    for (int b = 0; b < B; ++b) {
+      b200ms_result &rr = res[W.i0 + ids[b]];
+      if (skip[b]) continue;
+      const cplx *s = sv.data() + (size_t)b * 3, *t = sx.data() + (size_t)b * 3;
+      const cd wv(s[0].re, s[0].im), l1 = cd(s[1].re, s[1].im) / wv, a2(s[2].re, s[2].im);
+      const cd wx(t[0].re, t[0].im), w1x(t[1].re, t[1].im);
+      const cd l2 = (a2 + 2.0 * (w1x - l1 * wx)) / wv;  // f^2 d^2 lambda / df^2
+      const double f = freq[b];
+      const cd dl = l1 / f, d2l = l2 / (f * f);
+      const cd sn = nsorted[(size_t)b * k + q];  // sqrt(-lambda)
+      const cd ds = -dl / (2.0 * sn), d2s = -(d2l + 2.0 * ds * ds) / (2.0 * sn);
+      cd d2n = ps[b]->knorm * d2s;
+      if (!(resv[b] <= 100.0 * tol)) d2n = cd(std::nan(""), std::nan(""));
+      rr.d2n_dfreq2[2 * q] = d2n.real();
+      rr.d2n_dfreq2[2 * q + 1] = d2n.imag();
+      if (rr.d2n_residual) rr.d2n_residual[q] = resv[b];
+    }
+  }
+  S.reset_sigma();
 }
 
 template <typename T, typename C, typename P, typename PC>
@@ -938,9 +1095,17 @@ void solve_group(b200ms_handle *h, const std::vector<int> &ids, const Window &W,
     h->warm_B = B; h->warm_k = k; h->warm_len = S.len; h->warm_tsize = (int)sizeof(T);
     h->warm_valid = true;
   }
-  bool want_deriv = false;
-  for (int b = 0; b < B; ++b) want_deriv = want_deriv || res[W.i0 + ids[b]].dn_dfreq || res[W.i0 + ids[b]].dn_deps;
-  if (want_deriv) derivative_pass(h, S, ps, ids, W, prob, res, nsorted);
+  bool want_deriv = false, want_disp = false;
+  for (int b = 0; b < B; ++b) {
+    const b200ms_result &rb = res[W.i0 + ids[b]];
+    want_deriv = want_deriv || rb.dn_dfreq || rb.dn_deps || rb.d2n_dfreq2;
+    want_disp = want_disp || rb.d2n_dfreq2;
+  }
+  if (want_deriv) {
+    DerivArgs<T, C> da;
+    derivative_pass(h, S, ps, ids, W, prob, res, nsorted, da);
+    if (want_disp) dispersion_pass(h, S, ps, ids, W, prob, res, nsorted, lam, da);
+  }
   CUDA_CHECK(cudaEventRecord(h->ev1, h->stream));
   CUDA_CHECK(cudaEventSynchronize(h->ev1));
   float ms = 0.f;
@@ -1075,7 +1240,7 @@ extern "C" int b200ms_solve_batch(b200ms_handle *h, int nprob, const b200ms_prob
           res[i].eps_spec = s.eps_spec;
           res[i].is_complex = s.is_complex;
           std::string err = s.error;
-          if (res[i].status == B200MS_OK && (res[i].dn_dfreq || res[i].dn_deps) && (s.tensorial || s.relative || s.masked)) {
+          if (res[i].status == B200MS_OK && (res[i].dn_dfreq || res[i].dn_deps || res[i].d2n_dfreq2) && (s.tensorial || s.relative || s.masked)) {
             res[i].status = B200MS_ERR_UNSUPPORTED;
             err = s.tensorial ? "mode derivatives: tensorial problems (angled planes, off-diagonal eps) are not supported"
                   : s.relative ? "mode derivatives: the relative mode solver (basis fields) is not supported"

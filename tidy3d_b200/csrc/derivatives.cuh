@@ -163,4 +163,182 @@ __global__ void __launch_bounds__(256) deriv_map_kernel(DerivArgs<T, C> a) {
   for (int k = 0; k < 3; ++k) o[((size_t)k * N + g) * M + m] = d[k] * sc;
 }
 
+// ------------------------------------------------------------------------------------------------
+// Dispersion pass: the second frequency derivative of lambda (oracle/mode_dispersion.py is the float64 model).  In the scaled
+// direction ' = f d/df, with p = (exx, eyy, 1/ezz) of the solver frame and c the 1-D coefficients (A has degree <= 2 in each),
+//   A'v  = [A(c+c',p) - A(c-c',p)]/2 + [A(c,p+p') - A(c,p-p')]/2,
+//   A''v = A(c+c',p) + A(c-c',p) + A(c,p+p') + A(c,p-p') - 4 A(c,p) + [A(c+c'',p) - A(c-c'',p)]/2 + [A(c,p+p'') - A(c,p-p'')]/2
+//          + [A(c+c',p+p') - A(c+c',p-p') - A(c-c',p+p') + A(c-c',p-p')]/2
+// are exact with unit steps.  Per mode slot, phase 0 sums w^T v, w^T A'v and w^T A''v; phase 1 writes the projected right-hand
+// side r = -(A'v - beta v), beta = w^T A'v / w^T v, of the correction solve (A - lambda) x = r; phase 2 sums w^T x and
+// w^T A'x.  Then lambda'' = [w^T A''v + 2 (w^T A'x - lambda' w^T x)] / w^T v (the v-component of x drops out).
+// ------------------------------------------------------------------------------------------------
+
+// (A(c + sc dc, p + sp dp) v)(i, j) in double-complex arithmetic (the perturbations may be complex for a real operator)
+template <typename T, typename C, bool HAS_MU>
+struct PertSite {
+  const T *v1, *v2;
+  const C *fb;       // this problem's coefficient fields: exx, eyy, iez, mxx, myy, imz at fb + k N
+  const cplx *dp;    // this problem's [3][N] direction of (exx, eyy, iez), or null
+  double sp;
+  CoefRows<T> CX, CY;
+  int nx, ny;
+  size_t N;
+  __device__ __forceinline__ bool in(int ii, int jj) const { return ii >= 0 && ii < nx && jj >= 0 && jj < ny; }
+  __device__ __forceinline__ cplx V1(int ii, int jj) const { return in(ii, jj) ? to_cplx(ldg(v1 + (size_t)ii * ny + jj)) : mk(0.0, 0.0); }
+  __device__ __forceinline__ cplx V2(int ii, int jj) const { return in(ii, jj) ? to_cplx(ldg(v2 + (size_t)ii * ny + jj)) : mk(0.0, 0.0); }
+  __device__ __forceinline__ cplx cx(int w, int i) const { return to_cplx(CX(w, i)); }
+  __device__ __forceinline__ cplx cy(int w, int j) const { return to_cplx(CY(w, j)); }
+  __device__ __forceinline__ cplx fld(int k, size_t g) const {
+    cplx e = to_cplx(ldg(fb + (size_t)k * N + g));
+    if (dp) e += sp * ldg(dp + (size_t)k * N + g);
+    return e;
+  }
+  __device__ __forceinline__ cplx TT(int ii, int jj) const {
+    if (!in(ii, jj)) return mk(0.0, 0.0);
+    cplx acc = cx(0, ii) * V2(ii, jj) + cx(1, ii) * V2(ii + 1, jj) - cy(0, jj) * V1(ii, jj) - cy(1, jj) * V1(ii, jj + 1);
+    if (HAS_MU) acc = to_cplx(ldg(fb + 5 * N + (size_t)ii * ny + jj)) * acc;
+    return acc;
+  }
+  __device__ __forceinline__ cplx u(int i, int j) const {
+    if (!in(i, j)) return mk(0.0, 0.0);
+    const size_t g = (size_t)i * ny + j;
+    cplx uacc = cx(2, i) * (fld(0, g) * V1(i, j)) + cy(2, j) * (fld(1, g) * V2(i, j));
+    if (i > 0) uacc += cx(3, i) * (fld(0, g - ny) * V1(i - 1, j));
+    if (j > 0) uacc += cy(3, j) * (fld(1, g - 1) * V2(i, j - 1));
+    return -(fld(2, g) * uacc);
+  }
+  __device__ __forceinline__ void apply(int i, int j, cplx &p1, cplx &p2) const {
+    const size_t g = (size_t)i * ny + j;
+    const cplx t00 = TT(i, j);
+    const cplx q1 = cx(2, i) * t00 + cx(3, i) * TT(i - 1, j) + fld(1, g) * V2(i, j);
+    const cplx q2 = cy(2, j) * t00 + cy(3, j) * TT(i, j - 1) - fld(0, g) * V1(i, j);
+    const cplx u0 = u(i, j);
+    p1 = cx(0, i) * u0 + cx(1, i) * u(i + 1, j);
+    p2 = cy(0, j) * u0 + cy(1, j) * u(i, j + 1);
+    if (HAS_MU) {
+      p1 += to_cplx(ldg(fb + 4 * N + g)) * q2;
+      p2 -= to_cplx(ldg(fb + 3 * N + g)) * q1;
+    } else {
+      p1 += q2;
+      p2 -= q1;
+    }
+  }
+};
+
+// one operator evaluation of the difference formulas above: coefficient direction (0 none, 1 c', 2 c'') and step, field
+// direction (0 none, 1 p', 2 p'') and step, weight in A'v and in A''v
+struct DispTerm {
+  int cdir, pdir;
+  double sc, sp, w1, w2;
+};
+__constant__ DispTerm kDispTermsP[13] = {  // dispersive media
+    {1, 0, 1.0, 0.0, 0.5, 1.0},  {1, 0, -1.0, 0.0, -0.5, 1.0}, {0, 1, 0.0, 1.0, 0.5, 1.0},  {0, 1, 0.0, -1.0, -0.5, 1.0},
+    {0, 0, 0.0, 0.0, 0.0, -4.0}, {2, 0, 1.0, 0.0, 0.0, 0.5},   {2, 0, -1.0, 0.0, 0.0, -0.5}, {0, 2, 0.0, 1.0, 0.0, 0.5},
+    {0, 2, 0.0, -1.0, 0.0, -0.5}, {1, 1, 1.0, 1.0, 0.0, 0.5},  {1, 1, 1.0, -1.0, 0.0, -0.5}, {1, 1, -1.0, 1.0, 0.0, -0.5},
+    {1, 1, -1.0, -1.0, 0.0, 0.5}};
+__constant__ DispTerm kDispTermsC[5] = {  // nondispersive media: only the coefficients move
+    {1, 0, 1.0, 0.0, 0.5, 1.0}, {1, 0, -1.0, 0.0, -0.5, 1.0}, {0, 0, 0.0, 0.0, 0.0, -2.0}, {2, 0, 1.0, 0.0, 0.0, 0.5}, {2, 0, -1.0, 0.0, 0.0, -0.5}};
+
+template <typename T, typename C>
+struct DispArgs {
+  DerivArgs<T, C> d;    // Ritz vectors, coefficient fields, 1-D coefficients, f dc/df, metric and bend factors of the first-order pass
+  const T *c2x, *c2y;   // [B][4][n] f^2 d^2c/df^2 = 2 (f dc/df)^2 / c
+  const cplx *p1, *p2;  // [B][3][N] f dp/df and f^2 d^2p/df^2, or both null (nondispersive batch)
+  int q;                // mode slot
+  const T *x;           // phase 2: the correction, batched-vector layout
+  T *r;                 // phase 1: the right-hand side, batched-vector layout
+  const cplx *beta;     // phase 1: [B] w^T A'v / w^T v
+  cplx *partial;        // [B][nchunk][3]
+};
+
+// grid (nchunk, B), 256 threads; phases as described above
+template <typename T, typename C, bool HAS_MU>
+__global__ void __launch_bounds__(256) disp_scan_kernel(DispArgs<T, C> a, int phase) {
+  const int b = blockIdx.y, nx = a.d.nx, ny = a.d.ny;
+  const size_t N = (size_t)nx * ny;
+  const bool hp = a.p1 != nullptr;
+  const DispTerm *tab = hp ? kDispTermsP : kDispTermsC;
+  const int nterm = phase == 0 ? (hp ? 13 : 5) : (hp ? 4 : 2);
+  const T *vec = phase == 2 ? a.x + (size_t)b * 2 * N : a.d.vec + (size_t)a.q * a.d.vstride + (size_t)b * 2 * N;
+  const T *cxb = a.d.cx + (size_t)b * 4 * nx, *cyb = a.d.cy + (size_t)b * 4 * ny;
+  const T *d1x = a.d.dcx + (size_t)b * 4 * nx, *d1y = a.d.dcy + (size_t)b * 4 * ny;
+  const T *d2x = a.c2x + (size_t)b * 4 * nx, *d2y = a.c2y + (size_t)b * 4 * ny;
+  const cplx *p1 = hp ? a.p1 + (size_t)b * 3 * N : nullptr, *p2 = hp ? a.p2 + (size_t)b * 3 * N : nullptr;
+  const C *fb = a.d.fields + a.d.field_bstride * b;
+  const cplx beta = phase == 1 ? a.beta[b] : mk(0.0, 0.0);
+  cplx s0 = mk(0.0, 0.0), s1 = mk(0.0, 0.0), s2 = mk(0.0, 0.0);
+  for (size_t g = (size_t)blockIdx.x * 256 + threadIdx.x; g < N; g += (size_t)gridDim.x * 256) {
+    const int i = (int)(g / ny), j = (int)(g % ny);
+    cplx w1 = mk(0.0, 0.0), w2 = mk(0.0, 0.0);
+    if (phase != 1) deriv_cell<T, C, HAS_MU>(a.d, b, a.q, (const T *)nullptr, (const T *)nullptr, 0.0).w(i, j, w1, w2);
+    cplx a1x = mk(0.0, 0.0), a1y = mk(0.0, 0.0), a2x = mk(0.0, 0.0), a2y = mk(0.0, 0.0);
+#pragma unroll 1
+    for (int t = 0; t < nterm; ++t) {
+      const DispTerm tm = tab[t];
+      const T *dcx = tm.cdir == 1 ? d1x : (tm.cdir == 2 ? d2x : nullptr), *dcy = tm.cdir == 1 ? d1y : (tm.cdir == 2 ? d2y : nullptr);
+      const PertSite<T, C, HAS_MU> P{vec, vec + N, fb, tm.pdir == 1 ? p1 : (tm.pdir == 2 ? p2 : nullptr), tm.sp,
+                                     CoefRows<T>{cxb, dcx, tm.sc, nx}, CoefRows<T>{cyb, dcy, tm.sc, ny}, nx, ny, N};
+      cplx y1, y2;
+      P.apply(i, j, y1, y2);
+      a1x += tm.w1 * y1;
+      a1y += tm.w1 * y2;
+      a2x += tm.w2 * y1;
+      a2y += tm.w2 * y2;
+    }
+    const cplx e1 = to_cplx(ldg(vec + g)), e2 = to_cplx(ldg(vec + N + g));
+    if (phase == 1) {
+      T *rb = a.r + (size_t)b * 2 * N;
+      rb[g] = cast_to<T>(-(a1x - beta * e1));
+      rb[N + g] = cast_to<T>(-(a1y - beta * e2));
+      continue;
+    }
+    s0 += w1 * e1 + w2 * e2;
+    s1 += w1 * a1x + w2 * a1y;
+    s2 += w1 * a2x + w2 * a2y;
+  }
+  if (phase == 1) return;
+  __shared__ cplx red[3][256];
+  red[0][threadIdx.x] = s0;
+  red[1][threadIdx.x] = s1;
+  red[2][threadIdx.x] = s2;
+  __syncthreads();
+  for (int h = 128; h > 0; h >>= 1) {
+    if ((int)threadIdx.x < h)
+      for (int k = 0; k < 3; ++k) red[k][threadIdx.x] += red[k][threadIdx.x + h];
+    __syncthreads();
+  }
+  if (threadIdx.x < 3) a.partial[((size_t)b * gridDim.x + blockIdx.x) * 3 + threadIdx.x] = red[threadIdx.x][0];
+}
+
+// [B][3][N] f dp/df and f^2 d^2p/df^2 of p = (exx, eyy, iez) in the solver frame from d eps / df and d^2 eps / df^2 of the caller's
+// diagonal (in place: dp1 holds d eps / df on entry, dp2 d^2 eps / df^2).  Bend: exx = eps_xx / je, eyy = eps_yy / je,
+// ezz = je eps_zz; freq: [B] Hz.  iez' = -ezz' iez^2, iez'' = 2 ezz'^2 iez^3 - ezz'' iez^2.  PEC-valued cells: 0 (as eps_grad).
+template <typename C>
+__global__ void disp_fields_kernel(int nx, int ny, int B, const C *fields, size_t field_bstride, const double *jz_e, int jz_axis, int jz_len,
+                                   const double *freq, cplx *dp1, cplx *dp2) {
+  const size_t N = (size_t)nx * ny;
+  for (size_t t = (size_t)blockIdx.x * blockDim.x + threadIdx.x; t < (size_t)B * N; t += (size_t)gridDim.x * blockDim.x) {
+    const int b = (int)(t / N);
+    const size_t g = t % N;
+    const int i = (int)(g / ny), j = (int)(g % ny);
+    const double f = freq[b];
+    const C *fb = fields + field_bstride * b;
+    const double je = jz_e ? jz_e[(size_t)b * jz_len + (jz_axis == 0 ? i : j)] : 1.0;
+    cplx *d1 = dp1 + (size_t)b * 3 * N + g, *d2 = dp2 + (size_t)b * 3 * N + g;
+    const double pec = 0.9 * 1e8;
+    const cplx iz = to_cplx(ldg(fb + 2 * N + g));
+    for (int k = 0; k < 2; ++k) {
+      const bool is_pec = abs2(to_cplx(ldg(fb + (size_t)k * N + g))) >= pec * pec;
+      d1[(size_t)k * N] = is_pec ? mk(0.0, 0.0) : d1[(size_t)k * N] * (f / je);
+      d2[(size_t)k * N] = is_pec ? mk(0.0, 0.0) : d2[(size_t)k * N] * (f * f / je);
+    }
+    const cplx e1 = d1[2 * N] * (f * je), e2 = d2[2 * N] * (f * f * je);  // f ezz', f^2 ezz''
+    const bool is_pec = abs2(iz) * pec * pec <= 1.0;
+    const cplx iz2 = iz * iz;
+    d1[2 * N] = is_pec ? mk(0.0, 0.0) : -(e1 * iz2);
+    d2[2 * N] = is_pec ? mk(0.0, 0.0) : 2.0 * (e1 * e1) * (iz2 * iz) - e2 * iz2;
+  }
+}
+
 }  // namespace b200ms

@@ -434,13 +434,22 @@ class BatchSolver {
     capture_precondition_graph();
   }
 
-  // shift of the Krylov-side (reference) operator
+  // shift of the Krylov-side (reference) operator, in both precisions: sigma_ for the fp64 applies and sigma_p_ + B for the
+  // fine-level applies of the multigrid-precision FGMRES cycles (apply_true_u).  The multigrid keeps its own shift
+  // (set_sigma_mg), so a Krylov shift away from it -- the correction solves of the dispersion pass -- still refines
+  // towards A - sigma_Krylov.
   void set_sigma(const std::vector<cd> &s) {
     std::vector<T> h(B);
-    for (int b = 0; b < B; ++b) h[b] = from_cd<T>(s[b]);
+    std::vector<P> hp(B);
+    for (int b = 0; b < B; ++b) {
+      h[b] = from_cd<T>(s[b]);
+      hp[b] = from_cd<P>(s[b]);
+    }
     CUDA_CHECK(cudaMemcpyAsync(sigma_, h.data(), B * sizeof(T), cudaMemcpyHostToDevice, st_));
+    CUDA_CHECK(cudaMemcpyAsync(sigma_p_ + B, hp.data(), B * sizeof(P), cudaMemcpyHostToDevice, st_));
     CUDA_CHECK(cudaStreamSynchronize(st_));
   }
+  void reset_sigma() { set_sigma(sig_host_); }  // the eigen-solve's Krylov shift
   // shift of the multigrid operator (always the second-order diagonal-path operator A - sigma)
   void set_sigma_mg(const std::vector<cd> &s) {
     std::vector<P> hp(B);
@@ -1271,7 +1280,7 @@ class BatchSolver {
       apply_true(mode, x, rhs, y);
     } else {
       stats.stencil_applies++;
-      launch_stencil<P, PC>(lv[0], mode, x, rhs, y, lv[0].fields, cx_true_p_, cy_true_p_, sigma_p_);
+      launch_stencil<P, PC>(lv[0], mode, x, rhs, y, lv[0].fields, cx_true_p_, cy_true_p_, sigma_p_ + B);  // Krylov-side shift
     }
   }
   // z = M^-1 v.  For the multigrid-precision path the input is expected in lv[0].b already (the kernels that produce

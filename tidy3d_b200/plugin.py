@@ -219,6 +219,16 @@ def group_index(n_complex, freqs, step: float):
     f0 = f[1::3]
     inv = 1.0 / step
     n_group = center + (fwd - back) * inv * 0.5
-    c0 = 2.99792458e14
-    dispersion = (fwd * (inv + 1) + back * (inv - 1) - center * inv * 2) * f0.reshape(-1, 1) * (-1e18 * inv / c0**2)
+    dispersion = (fwd * (inv + 1) + back * (inv - 1) - center * inv * 2) * f0.reshape(-1, 1) * (-1e18 * inv / C0_UM**2)
     return f0, np.asarray(n_complex)[1::3], n_group, dispersion
+
+
+C0_UM = 2.99792458e14  # speed of light in um/s, the unit of the dispersion formula of monitor_data.py:1542-1548
+
+
+def dispersion_of(freq, dn_dfreq, d2n_dfreq2):
+    """Group-velocity dispersion (ps/(nm km)) from analytic frequency derivatives of n_eff + i k_eff
+    (``compute_modes_batch(..., derivatives=("freq2",))``): D = -1e18 f^2 (2 Re n' + f Re n'') / c0^2, the step -> 0 limit of
+    the three-point formula of ``group_index``.  ``freq`` broadcasts against the derivatives (e.g. shape (F, 1) with (F, M))."""
+    f = np.asarray(freq, float)
+    return -1e18 * f**2 * (2 * np.real(dn_dfreq) + f * np.real(d2n_dfreq2)) / C0_UM**2

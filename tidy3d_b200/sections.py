@@ -90,6 +90,15 @@ class Medium:
         h = 1e-4 * freq
         return (self.tensor(freq + h) - self.tensor(freq - h)) / (2 * h)
 
+    def d2tensor_dfreq2(self, freq: float) -> np.ndarray:
+        """d^2 eps / df^2 (1/Hz^2) of the 3x3 tensor: zero for a constant medium, a second central difference of ``eps(f)`` for a
+        dispersive one.  The relative step is 1e-3: the roundoff of a second difference grows like eps_mach / step^2 (1e-8
+        relative at 1e-4), its truncation error like step^2."""
+        if not callable(self.eps):
+            return np.zeros((3, 3), dtype=complex)
+        h = 1e-3 * freq
+        return (self.tensor(freq + h) - 2 * self.tensor(freq) + self.tensor(freq - h)) / (h * h)
+
 
 def site_medium_from_masks(shape: Tuple[int, int], masks: Sequence[Tuple[np.ndarray, int]]) -> np.ndarray:
     """(3, Nx, Ny) uint16 site map from per-structure inside-masks, drawn in structure order like epsilon_on_grid
@@ -151,10 +160,11 @@ class Section:
             raise ValueError("Mismatch between 'coords' and 'site_medium' shapes.")
         return sm
 
-    def pack(self, freq: float, shape: Optional[Tuple[int, int]] = None, dispersion: bool = False):
+    def pack(self, freq: float, shape: Optional[Tuple[int, int]] = None, dispersion: bool = False, second: bool = False):
         """ctypes ``b200ms_section`` for one frequency plus the arrays it points to (kept alive by the caller).  ``shape`` =
         (Nx, Ny) of the plane, needed to check ``site_medium``.  ``dispersion``: also pass every medium's d eps / df
-        (``deps_table``), the material term of the mode derivatives."""
+        (``deps_table``), the material term of the mode derivatives; ``second``: also every medium's d^2 eps / df^2
+        (``d2eps_table``), the material term of the second frequency derivative."""
         media, ids = self._media()
         n = len(self.structures)
         rects = np.zeros((n, 4), dtype=np.float64)
@@ -201,4 +211,8 @@ class Section:
         if dispersion and any(callable(m.eps) for m in media):
             dtable = np.ascontiguousarray([m.dtensor_dfreq(freq).ravel() for m in media], dtype=np.complex128)
             st.deps_table = dtable.view(np.float64).ctypes.data_as(_cabi._dp)
-        return st, (rects, med, table, kinds, pstart, pxy, site, dtable)
+        d2table = None
+        if second and any(callable(m.eps) for m in media):
+            d2table = np.ascontiguousarray([m.d2tensor_dfreq2(freq).ravel() for m in media], dtype=np.complex128)
+            st.d2eps_table = d2table.view(np.float64).ctypes.data_as(_cabi._dp)
+        return st, (rects, med, table, kinds, pstart, pxy, site, dtable, d2table)

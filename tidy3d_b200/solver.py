@@ -104,16 +104,24 @@ def compute_modes_batch(
     (n_eff + f Re(dn/df), what ``ModeData._group_index_post_process`` approximates from three solves) to the info dict;
     ``"eps"`` adds ``dn_deps`` (3, Nx, Ny, M): d(n_eff + i k_eff) / d eps_{xx,yy,zz} of ``eps_cross`` at every Yee site (PML stretch
     held fixed).  Material dispersion enters ``dn_dfreq`` through a problem's ``eps_dfreq=`` (d eps_cross / df) or, for a
-    ``section``, through the media whose ``eps`` is a callable.  ``n_complex`` and the fields do not change.
+    ``section``, through the media whose ``eps`` is a callable.  ``"freq2"`` adds the group-velocity dispersion from one
+    correction solve per mode on top of the same solve: ``d2n_dfreq2`` (d^2(n_eff + i k_eff)/df^2, 1/Hz^2; NaN for a mode whose
+    correction solve stopped above 100 x the inner tolerance), ``d2n_residual`` (that solve's final relative residual) and
+    ``dispersion`` (ps/(nm km), ``plugin.dispersion_of``: the step -> 0 limit of ``plugin.group_index``), and implies
+    ``"freq"``; its material term comes from a problem's ``eps_dfreq=`` and ``eps_d2freq=`` (d^2 eps_cross / df^2) or a
+    section's callable media.  ``n_complex``, the fields, ``dn_dfreq`` and ``dn_deps`` do not change.
     """
     post = tuple(post or ())
     unknown = set(post) - {"gauge", "normalize", "flux", "overlaps"}
     if unknown:
         raise ValueError(f"unknown post-processing step(s): {sorted(unknown)}")
     derivatives = tuple(derivatives or ())
-    unknown = set(derivatives) - {"freq", "eps"}
+    unknown = set(derivatives) - {"freq", "eps", "freq2"}
     if unknown:
         raise ValueError(f"unknown derivative(s): {sorted(unknown)}")
+    second = "freq2" in derivatives
+    if second and "freq" not in derivatives:
+        derivatives = derivatives + ("freq",)
     post_flags = (1 if "gauge" in post else 0) | (2 if "normalize" in post else 0)
     packed, cache = [], {}
     for p in problems:
@@ -138,7 +146,7 @@ def compute_modes_batch(
             mu_cross=p.get("mu_cross"), target_override=target_override,
             incidence=(split is not None or p.get("mu_cross") is not None),  # solver.py:93
             post=post_flags, grid_correction=p.get("grid_correction"), plane_bounds=p.get("plane_bounds"),
-            eps_dfreq=p.get("eps_dfreq"), derivatives="freq" in derivatives,
+            eps_dfreq=p.get("eps_dfreq"), derivatives="freq" in derivatives, eps_d2freq=p.get("eps_d2freq"), second=second,
         )  # fmt: skip
         if split is None and section is None:
             cache[key] = pk.eps
@@ -151,11 +159,12 @@ def compute_modes_batch(
         packed.append(pk)
     h = handle or get_handle(device)  # after input validation: argument errors do not need a GPU
     with h.lock:
-        dkw = dict(want_dfreq="freq" in derivatives, want_deps="eps" in derivatives) if derivatives else {}
+        dkw = dict(want_dfreq="freq" in derivatives, want_deps="eps" in derivatives, want_d2freq=second) if derivatives else {}
         rc, fields, ncs, results = h.solve_batch(packed, want_fields, fields_ptrs, want_flux=("flux" in post or "normalize" in post),
                                                  want_overlaps="overlaps" in post, **dkw)
         flux_out, te_out, ov_out = h.last_flux, h.last_te, h.last_overlaps
         dfreq_out, deps_out = (h.last_dn_dfreq, h.last_dn_deps) if derivatives else ([], [])
+        d2_out, d2res_out = (h.last_d2n_dfreq2, h.last_d2n_residual) if second else ([], [])
         err = h.last_error() if rc != _cabi.OK else ""
     if rc != _cabi.OK:
         bad = [i for i in range(len(packed)) if results[i].status != _cabi.OK]
@@ -182,6 +191,12 @@ def compute_modes_batch(
             infos[-1]["n_group"] = ncs[i].real + float(packed[i].struct.freq) * dfreq_out[i].real
         if deps_out:
             infos[-1]["dn_deps"] = deps_out[i]
+        if d2_out:
+            from .plugin import dispersion_of  # noqa: PLC0415  (plugin imports this module)
+
+            infos[-1]["d2n_dfreq2"] = d2_out[i]
+            infos[-1]["d2n_residual"] = d2res_out[i]
+            infos[-1]["dispersion"] = dispersion_of(float(packed[i].struct.freq), dfreq_out[i], d2_out[i])
     return (out, infos) if return_info else out
 
 

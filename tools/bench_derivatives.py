@@ -1,9 +1,12 @@
-"""Group index three ways on the headline workload (Si strip 512x512, 4 modes), alternated in one process:
-  plain   -- one solve per frequency, no derivatives;
-  analytic -- one solve per frequency with derivatives=("freq",) (n_group from the left eigenvector);
-  fd3     -- three solves per frequency at f(1 -/+ step) and f, n_group by plugin.group_index (the reference's path).
-Prints one JSON line: solves/s, frequencies-with-group-index/s, the device time the derivative pass adds per problem and the
-pass's algorithmic bytes against the 3.35 TB/s HBM3 data-sheet figure, with the card name and power limit read in the same run.
+"""Group index and dispersion on the headline workload (Si strip 512x512, 4 modes), alternated in one process:
+  plain        -- one solve per frequency, no derivatives;
+  analytic     -- one solve per frequency with derivatives=("freq",) (n_group from the left eigenvector);
+  analytic_gvd -- one solve per frequency with derivatives=("freq2",) (n_group and the dispersion, one correction solve per mode);
+  fd3          -- three solves per frequency at f(1 -/+ step) and f, n_group and dispersion by plugin.group_index (the reference's path).
+Prints one JSON line: solves/s, frequencies-with-group-index/s, frequencies-with-dispersion/s, the device time the derivative
+and dispersion passes add per problem, the correction solves' inner iterations per mode, the largest differences against fd3 and
+the derivative pass's algorithmic bytes against the 3.35 TB/s HBM3 data-sheet figure, with the card name and power limit read
+in the same run.
 
     python tools/bench_derivatives.py [--nf 64] [--rounds 2] [--n 512] [--out results/bench_derivatives.json]
 """
@@ -55,13 +58,15 @@ def main():
     arms = {
         "plain": lambda: compute_modes_batch(probs(wl.freqs), handle=h, want_fields=False, return_info=True),
         "analytic": lambda: compute_modes_batch(probs(wl.freqs), handle=h, want_fields=False, return_info=True, derivatives=("freq",)),
+        "analytic_gvd": lambda: compute_modes_batch(probs(wl.freqs), handle=h, want_fields=False, return_info=True, derivatives=("freq2",)),
         "fd3": lambda: compute_modes_batch(probs(f3), handle=h, want_fields=False, return_info=True),
     }
     for fn in arms.values():  # warm-up of every shape
         fn()
     t = {k: [] for k in arms}
     dev = {k: [] for k in arms}
-    ng = {}
+    ng, disp = {}, {}
+    inner = {k: [] for k in arms}
     for _ in range(a.rounds):
         for k, fn in arms.items():
             torch.cuda.synchronize()
@@ -70,26 +75,40 @@ def main():
             torch.cuda.synchronize()
             t[k].append(time.perf_counter() - t0)
             dev[k].append(h.last_stats()["device_ms"])
+            inner[k].append(h.last_stats()["inner_iters"])
             if k == "analytic":
                 ng["analytic"] = np.array([i["n_group"] for i in infos])
+            if k == "analytic_gvd":
+                disp["analytic_gvd"] = np.array([i["dispersion"] for i in infos])
+                res_gvd = np.array([i["d2n_residual"] for i in infos])
             if k == "fd3":
-                ng["fd3"] = plugin.group_index(np.array([o[1] for o in out]), f3, a.step)[2]
-    nsolve = {"plain": a.nf, "analytic": a.nf, "fd3": 3 * a.nf}
+                _, _, ng["fd3"], disp["fd3"] = plugin.group_index(np.array([o[1] for o in out]), f3, a.step)
+    nsolve = {"plain": a.nf, "analytic": a.nf, "analytic_gvd": a.nf, "fd3": 3 * a.nf}
     N, M = a.n * a.n, wl.mode_spec.num_modes
     # one derivative pass reads, per (problem, mode), the real fp64 Ritz vector (2N x 8 B) and the three coefficient fields
     # (exx, eyy, 1/ezz: 3N x 8 B; shared by the sweep, counted once per mode pass as they are re-read)
     bytes_pass = a.nf * M * (2 * N * 8 + 3 * N * 8)
     extra_ms = (np.median(dev["analytic"]) - np.median(dev["plain"]))
+    gvd_ms = (np.median(dev["analytic_gvd"]) - np.median(dev["analytic"]))
+    # the eigen-solves of the two arms are bit-identical, so the difference of the summed inner iterations is the correction
+    # solves' (per problem: the slowest problem of its device batch, as for the eigen-solve's own counters)
+    corr_iters = (np.median(inner["analytic_gvd"]) - np.median(inner["analytic"])) / (a.nf * M)
     res = dict(
         card=card(), workload=f"headline {a.n}x{a.n}, {M} modes, {a.nf} frequencies", rounds=a.rounds,
         solves_per_s={k: nsolve[k] / float(np.median(v)) for k, v in t.items()},
         freqs_with_group_index_per_s={"analytic": a.nf / float(np.median(t["analytic"])), "fd3": a.nf / float(np.median(t["fd3"]))},
+        freqs_with_dispersion_per_s={"analytic_gvd": a.nf / float(np.median(t["analytic_gvd"])), "fd3": a.nf / float(np.median(t["fd3"]))},
         device_ms_median={k: float(np.median(v)) for k, v in dev.items()},
         derivative_pass_device_ms_per_problem=float(extra_ms / a.nf),
+        dispersion_pass_device_ms_per_problem=float(gvd_ms / a.nf),
+        correction_inner_iters_per_mode=float(corr_iters),
+        correction_residual_max=float(res_gvd.max()),
         derivative_pass_bytes=bytes_pass,
         derivative_pass_bw_TBps=float(bytes_pass / max(extra_ms, 1e-9) / 1e9),
         hbm_datasheet_TBps=3.35,
         n_group_max_abs_diff_analytic_vs_fd3=float(np.abs(ng["analytic"] - ng["fd3"]).max()),
+        dispersion_max_abs_diff_analytic_gvd_vs_fd3_ps_per_nm_km=float(np.abs(disp["analytic_gvd"] - disp["fd3"]).max()),
+        dispersion_range_fd3_ps_per_nm_km=[float(disp["fd3"].min()), float(disp["fd3"].max())],
     )  # fmt: skip
     line = json.dumps(res)
     print(line)
