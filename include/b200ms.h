@@ -256,8 +256,9 @@ typedef struct {
   int stencil_pair_rows; /* rows marched per CTA by the pair kernel (rounded to 6 m - 3); 0 (default) = chosen per level from the
                             number of resident CTAs */
   int transfer_vec;      /* multigrid transfers: bit 0 = the prolongation reads / writes its four fine values as one 128-bit access (fp32 vectors,
-                            nyf % 4 == 0); bit 1 = the restriction reads each fine row of its patch as aligned 64-bit pairs when the patch is
-                            contiguous */
+                            nyf % 4 == 0); bit 1 = the restriction reads packed lists of up to four entries; bit 2 (with bit 1) = on levels the
+                            TMA pair kernel covers in one strip, the residual is restricted inside the residual kernel and never stored (same
+                            results bit for bit).  Default 7; 3 gives the separate residual and restriction kernels */
   int tensor_mg_cycles;  /* tensorial path: V-cycles (defect correction on the multigrid operator) per application of the E-block inverse inside
                             the block preconditioner; 0 = mg_cycles.  Default 3 (see csrc/solver.cuh mg_cycles_ and tools/proto_tensor.py) */
 } b200ms_options;
@@ -351,7 +352,9 @@ int b200ms_debug_post_tables_bounded(const double *coords, int n, int sym, doubl
  *                  in the multigrid precision (mode + 16 selects it on level 0 as well): mode 0 apply, 1 residual,
  *                  2 stored-diagonal Jacobi sweep (x = in, rhs = in2), 3 omega D^-1 in2, 4 two sweeps from zero on in2.
  *                  Vectors have 2 nx_l ny_l elements per problem.
- *   what 1: one preconditioner application out = M^-1 in (the multigrid V-cycle; tensorial: the block preconditioner).
+ *   what 1: one preconditioner application out = M^-1 in (the multigrid V-cycle; tensorial: the block preconditioner);
+ *           *iters (when not NULL) gets a bit mask of the levels whose residual was restricted inside the residual kernel
+ *           (transfer_vec bit 2).
  *   what 2: out = (A - sigma)^-1 in by the inner solver of the eigen-iteration, to the handle's inner_tol; *iters gets its
  *           Arnoldi steps, relres[nprob] the final relative residual of every problem. */
 int b200ms_debug_batch(b200ms_handle *h, int nprob, const b200ms_problem *probs, int what, int level, int mode,

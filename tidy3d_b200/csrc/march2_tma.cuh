@@ -11,6 +11,14 @@
 // __syncthreads that ends the step which consumed it (the march needs that barrier anyway), so no "empty" barriers exist.
 // Requirements beyond the register version: ny % 4 == 0 (16-byte aligned row slices).  MODE_JACOBI_D0 stays with the register
 // version.  A wait that does not complete within ~2^24 polls traps instead of hanging the device.
+//
+// MODE_RESID_RESTRICT: the residual followed by the restriction to the next coarser level, without storing the fine residual.
+// A CTA owns the coarse rows [I0, I0 + rows) (rows = coarse rows here) and marches the fine rows their restriction lists
+// reach (Ex: x-edge lists, Ey: x-node lists); the fine rows two neighbouring CTAs both need are computed by both.  Each
+// residual row goes to a ring of kRrRing rows in shared memory, and a coarse row is formed as soon as the last fine row
+// of its lists is there, by restrict4_kernel's expression in restrict4_kernel's order (csrc/kernels.cuh).  One strip per
+// row (ny <= 2 kM2MaxW), packed lists on all four axes; the host checks that no coarse row needs a fine row older than the
+// ring holds (resid_restrict_plan in csrc/solver.cuh).
 #pragma once
 
 namespace b200ms {
@@ -53,14 +61,22 @@ struct M2TmaArrays {
   static constexpr int n = 5 + (MODE != MODE_APPLY ? 2 : 0) + (MODE == MODE_JACOBI_D ? 2 : 0);
 };
 
+constexpr int kRrRing = 8;  // residual rows held for the restriction (power of two)
+
+// dynamic shared memory of MODE_RESID_RESTRICT beyond the row ring: residual ring [kRrRing][2][ny] floats, then the fine-row
+// range of the CTA and the last fine row of each of its coarse rows
+inline size_t rr_smem_extra(int ny) { return (size_t)kRrRing * 2 * ny * sizeof(float) + (2 + kM2MaxSteps) * sizeof(int); }
+
 template <int MODE, int D>
 __global__ void __launch_bounds__(kM2MaxW, 2) stencil_march2_tma_kernel(StencilArgs<float, float> a, int rows) {
-  static_assert(MODE == MODE_APPLY || MODE == MODE_RESID || MODE == MODE_JACOBI_D, "TMA pair kernel: apply / residual / stored-diagonal sweep");
+  static_assert(MODE == MODE_APPLY || MODE == MODE_RESID || MODE == MODE_JACOBI_D || MODE == MODE_RESID_RESTRICT,
+                "TMA pair kernel: apply / residual / stored-diagonal sweep / residual + restriction");
   static_assert(kM2Unroll % D == 0, "ring depth must divide the unroll factor");
   using T = float;
   using V = float2;
   constexpr bool HAS_RHS = (MODE != MODE_APPLY);
   constexpr bool DSTORED = (MODE == MODE_JACOBI_D);
+  constexpr bool RESTR = (MODE == MODE_RESID_RESTRICT);
   constexpr int NARR = M2TmaArrays<MODE>::n;
   __shared__ T sB[2][kM2MaxW + 2], sV[2][kM2MaxW + 2], sU[2][kM2MaxW + 2], sTt[2][kM2MaxW + 2];
   __shared__ RowCoef<T> sX[kM2MaxSteps + 2];
@@ -77,12 +93,36 @@ __global__ void __launch_bounds__(kM2MaxW, 2) stencil_march2_tma_kernel(StencilA
   const int q0 = (int)blockIdx.x * (W - 2);  // first column pair of the strip
   const int q = q0 + c;
   const int gj = 2 * q;
-  const int i0 = blockIdx.y * rows;
-  const int iend = (i0 + rows < nx) ? i0 + rows : nx;
-  const int k0 = i0 - 3;
-  const int nsteps = rows + 3;
+  int i0 = blockIdx.y * rows;
+  int iend = (i0 + rows < nx) ? i0 + rows : nx;
+  int k0 = i0 - 3;
+  int nsteps = rows + 3;
   const bool colv = q < npairs;
   const bool outc = colv && (c >= 1 || blockIdx.x == 0) && (c <= W - 2 || q == npairs - 1);
+  // MODE_RESID_RESTRICT: the CTA's coarse rows [I0, I1) and the fine rows [i0, iend) their restriction lists reach
+  T *sRes = nullptr;
+  int *sRng = nullptr;
+  int I0 = 0, I1 = 0;
+  if constexpr (RESTR) {
+    sRes = reinterpret_cast<T *>(m2_ring_raw + (size_t)D * NARR * W * sizeof(V));
+    sRng = reinterpret_cast<int *>(sRes + (size_t)kRrRing * 2 * ny);
+    I0 = blockIdx.y * rows;
+    I1 = min(I0 + rows, a.tr->nxc);
+    if (c == 0) { sRng[0] = nx; sRng[1] = -1; }
+    __syncthreads();
+    if (c < I1 - I0) {
+      const int4 xe = __ldg(reinterpret_cast<const int4 *>(a.tr->xe.r4 + I0 + c)), xn = __ldg(reinterpret_cast<const int4 *>(a.tr->xn.r4 + I0 + c));
+      const int hi = max(xe.w, xn.w);  // packed lists ascend and repeat their last index
+      sRng[2 + c] = hi;
+      atomicMin(&sRng[0], min(xe.x, xn.x));
+      atomicMax(&sRng[1], hi);
+    }
+    __syncthreads();
+    i0 = sRng[0];
+    iend = sRng[1] + 1;
+    nsteps = kM2Unroll * ((iend - i0 + 3 + kM2Unroll - 1) / kM2Unroll);
+    k0 = i0 - 3;
+  }
   const T *x1 = a.x + (size_t)b * 2 * N, *x2 = x1 + N;
   const T *fb = a.fields + a.field_bstride * b;
   const T *exx = fb, *eyy = fb + N, *iez = fb + 2 * (size_t)N;
@@ -94,7 +134,8 @@ __global__ void __launch_bounds__(kM2MaxW, 2) stencil_march2_tma_kernel(StencilA
   const V zV = {zT, zT};
   const int wcopy = (npairs - q0 < W) ? npairs - q0 : W;  // column pairs of this strip that exist
   const unsigned nbytes = (unsigned)wcopy * (unsigned)sizeof(V);
-  const int raw_lo = (i0 - 1 > 0) ? i0 - 1 : 0, raw_hi = (i0 + rows < nx - 1) ? i0 + rows : nx - 1;
+  const int raw_lo = (i0 - 1 > 0) ? i0 - 1 : 0;
+  const int raw_hi = RESTR ? min(iend, nx - 1) : (i0 + rows < nx - 1) ? i0 + rows : nx - 1;
 
   // lanes 0 .. NARR-1 of warp 0 each own one array: lane 0 arms the stage of step jj (expect_tx = the bytes of that step), then
   // every owner lane issues the bulk copy of its array's row slice
@@ -140,6 +181,34 @@ __global__ void __launch_bounds__(kM2MaxW, 2) stencil_march2_tma_kernel(StencilA
     for (int s = 0; s < D; ++s)
       if (s < nsteps) issue(s, s);
   }
+
+  // coarse row I of both components out of the residual ring: restrict4_kernel's sums in its order, with its contractions
+  int nI = I0;
+  auto restrict_row = [&](int I) {
+    const TransferArgs &t = *a.tr;
+    const int nyc = t.nyc;
+    const size_t Nc = (size_t)t.nxc * nyc;
+    for (int o = c; o < 2 * nyc; o += W) {
+      const int comp = o >= nyc ? 1 : 0, J = o - comp * nyc;
+      const RList4 *tx = comp == 0 ? t.xe.r4 : t.xn.r4, *ty = comp == 0 ? t.yn.r4 : t.ye.r4;
+      const int4 xi = __ldg(reinterpret_cast<const int4 *>(tx + I)), yi = __ldg(reinterpret_cast<const int4 *>(ty + J));
+      const float4 xw = __ldg(reinterpret_cast<const float4 *>(tx + I) + 1), yw = __ldg(reinterpret_cast<const float4 *>(ty + J) + 1);
+      const int ix[4] = {xi.x, xi.y, xi.z, xi.w}, iy[4] = {yi.x, yi.y, yi.z, yi.w};
+      const float wx[4] = {xw.x, xw.y, xw.z, xw.w}, wy[4] = {yw.x, yw.y, yw.z, yw.w};
+      T acc = 0.0f;
+#pragma unroll
+      for (int p = 0; p < 4; ++p) {
+        const T *row = sRes + (size_t)(ix[p] & (kRrRing - 1)) * 2 * ny + comp * ny;
+        T racc = 0.0f;
+#pragma unroll
+        for (int qq = 0; qq < 4; ++qq) racc = __fmaf_rn(wy[qq], row[iy[qq]], racc);
+        acc = __fmaf_rn(wx[p], racc, acc);
+      }
+      if ((comp == 0 && t.mask_y && J == 0 && nyc > 1) || (comp == 1 && t.mask_x && I == 0 && t.nxc > 1)) acc = 0.0f;
+      a.coarse[((size_t)b * 2 + comp) * Nc + (size_t)I * nyc + J] = acc;
+    }
+  };
+  (void)restrict_row;
 
   V a1 = zV, b1 = zV, v11 = zV, v21 = zV, a0 = zV, b0 = zV, v10 = zV, v20 = zV, ie1 = zV;
   V u0 = zV, t0 = zV, tm = zV;
@@ -196,6 +265,10 @@ __global__ void __launch_bounds__(kM2MaxW, 2) stencil_march2_tma_kernel(StencilA
           stg2(y1 + g, o1x, o1y); stg2(y2 + g, o2x, o2y);
         } else if (MODE == MODE_RESID) {
           stg2(y1 + g, cr1.x - o1x, cr1.y - o1y); stg2(y2 + g, cr2.x - o2x, cr2.y - o2y);
+        } else if (RESTR) {
+          T *rr = sRes + (size_t)(k & (kRrRing - 1)) * 2 * ny + gj;
+          *reinterpret_cast<V *>(rr) = make_float2(cr1.x - o1x, cr1.y - o1y);
+          *reinterpret_cast<V *>(rr + ny) = make_float2(cr2.x - o2x, cr2.y - o2y);
         } else {
           stg2(y1 + g, v10.x + cd1.x * (cr1.x - o1x), v10.y + cd1.y * (cr1.y - o1y));
           stg2(y2 + g, v20.x + cd2.x * (cr2.x - o2x), v20.y + cd2.y * (cr2.y - o2y));
@@ -208,6 +281,13 @@ __global__ void __launch_bounds__(kM2MaxW, 2) stencil_march2_tma_kernel(StencilA
       __syncthreads();
       // every thread has read stage `stage`: refill it with the rows of step j + D
       if (c < NARR && j + D < nsteps) issue(j + D, stage);
+      if constexpr (RESTR) {
+        // the coarse rows whose last fine row is row k (the ring still holds their first one: resid_restrict_plan)
+        while (nI < I1 && k >= sRng[2 + nI - I0]) {
+          restrict_row(nI);
+          ++nI;
+        }
+      }
     }
   }
 }

@@ -117,6 +117,8 @@ class BatchSolver {
     P *x = nullptr, *b = nullptr, *r = nullptr, *tmp = nullptr;
     P *dinv = nullptr;  // omega / diag(A_l - sigma), [B][2][N]
     TransferArgs tr;  // to the next coarser level
+    const TransferArgs *tr_dev = nullptr;  // device copy of tr
+    int rr_rows = 0;  // coarse rows per CTA of the fused residual + restriction (csrc/march2_tma.cuh); 0: separate kernels
   };
 
   BatchSolver(Arena &arena, cudaStream_t stream, const b200ms_options &opt) : arena_(arena), st_(stream), opt_(opt) {
@@ -196,6 +198,7 @@ class BatchSolver {
         transfer_sizes(plan_.try_[l], ints, dbls);
         sz.add<int>(ints + 64);
         sz.add<double>(dbls + 64);
+        sz.add<TransferArgs>(1);
       }
     }
     sz.add<T>((size_t)(m + 1) * vstride);        // outer basis
@@ -331,6 +334,7 @@ class BatchSolver {
       upload_transfer(plan_.trx[l].edge, t.xe);
       upload_transfer(plan_.try_[l].node, t.yn);
       upload_transfer(plan_.try_[l].edge, t.ye);
+      lv[l].tr_dev = up(std::vector<TransferArgs>{t});
       // site types: exx (e,n)  eyy (n,e)  ezz (n,n)  mxx (n,e)  myy (e,n)  mzz (e,e)
       const Transfer1DDev *fx[6] = {&t.xe, &t.xn, &t.xn, &t.xn, &t.xe, &t.xe};
       const Transfer1DDev *fy[6] = {&t.yn, &t.ye, &t.yn, &t.ye, &t.yn, &t.ye};
@@ -512,6 +516,17 @@ class BatchSolver {
     March2Fn fn = nullptr;
     int stages = 0, narr = 0, id = 0;  // stages > 0: TMA version with that ring depth
   };
+  // the most recent pair-kernel launch, kept so that the V-cycle graph can redirect the output of its last sweep
+  struct M2Launch {
+    March2Fn fn = nullptr;
+    dim3 grd;
+    int W = 0;
+    size_t smem = 0;
+    StencilArgs<float, float> a;
+    int rows = 0;
+    long seq = -1;  // stats.launches when it was launched
+  };
+  M2Launch last_m2_;
   March2Pick march2_pick(int md, int ny) const {
     March2Pick p;
     const int sp = opt_.stencil_pair;
@@ -566,7 +581,9 @@ class BatchSolver {
   // occupancy queries and attribute changes happen here, before the V-cycle is captured into a CUDA graph
   void prime_march2() {
     if constexpr (std::is_same<P, float>::value && std::is_same<PC, float>::value) {
-      for (const Level &v : lv) {
+      for (size_t l = 0; l < lv.size(); ++l) {
+        Level &v = lv[l];
+        v.rr_rows = 0;
         if (!march2_eligible(v)) continue;
         int W = 0, nstrips = 0;
         march2_strips(v.ny, W, nstrips);
@@ -574,7 +591,113 @@ class BatchSolver {
           const March2Pick p = march2_pick(md, v.ny);
           if (p.fn) march2_resident(p, md, W);
         }
+        if (l + 1 < lv.size()) v.rr_rows = resid_restrict_plan((int)l, W, nstrips);
       }
+    }
+  }
+  March2Pick resid_restrict_pick(int ny) const {
+    March2Pick p = march2_pick(MODE_RESID, ny);
+    if (p.stages == 3) p.fn = stencil_march2_tma_kernel<MODE_RESID_RESTRICT, 3>;
+    else if (p.stages == 2) p.fn = stencil_march2_tma_kernel<MODE_RESID_RESTRICT, 2>;
+    else p.fn = nullptr;
+    p.id = 32 + p.stages;
+    return p;
+  }
+  // Coarse rows per CTA of the fused residual + restriction on level l (csrc/march2_tma.cuh), or 0 where it does not apply:
+  // the TMA pair kernel in one strip, packed restriction lists of 1 .. 4 ascending entries, every coarse row within reach of
+  // the residual ring, at most kM2MaxSteps - 3 fine rows per CTA.  Where it applies, the results are those of the residual
+  // kernel followed by restrict4_kernel, bit for bit.
+  int resid_restrict_plan(int l, int W, int nstrips) {
+    const Level &v = lv[l];
+    const TransferArgs &t = v.tr;
+    if (!(opt_.transfer_vec & 4) || !(opt_.transfer_vec & 2) || opt_.transfer_tiled || nstrips != 1 || v.ny > 2 * kM2MaxW) return 0;
+    if (!t.xn.r4 || !t.xe.r4 || !t.yn.r4 || !t.ye.r4) return 0;
+    const March2Pick p = resid_restrict_pick(v.ny);
+    if (!p.fn) return 0;
+    const Transfer1D &xe = plan_.trx[l].edge, &xn = plan_.trx[l].node;
+    const int nxc = t.nxc;
+    std::vector<int> lo(nxc), hi(nxc);
+    for (int I = 0; I < nxc; ++I) {
+      int mn = v.nx, mx = -1;
+      for (const Transfer1D *q : {&xe, &xn}) {
+        const int k0 = q->r_ptr[I], k1 = q->r_ptr[I + 1];
+        if (k1 - k0 < 1 || k1 - k0 > 4) return 0;
+        for (int kk = k0 + 1; kk < k1; ++kk)
+          if (q->r_idx[kk] < q->r_idx[kk - 1]) return 0;
+        mn = std::min(mn, q->r_idx[k0]);
+        mx = std::max(mx, q->r_idx[k1 - 1]);
+      }
+      lo[I] = mn;
+      hi[I] = mx;
+    }
+    // per CTA of `ncr` coarse rows: a coarse row is formed once every earlier one is, at the fine step max(hi) so far; the
+    // ring must still hold its first fine row then.  Fine rows per CTA: max(hi) - min(lo) + 1.  Returns the most row steps
+    // of a CTA (fine rows + 3, rounded up to the unroll factor), or 0 when some CTA does not fit.
+    auto max_steps = [&](int ncr) {
+      int worst = 0;
+      for (int I0 = 0; I0 < nxc; I0 += ncr) {
+        int run = -1, mn = v.nx;
+        for (int I = I0; I < std::min(nxc, I0 + ncr); ++I) {
+          run = std::max(run, hi[I]);
+          mn = std::min(mn, lo[I]);
+          if (run - lo[I] + 1 > kRrRing - 1) return 0;
+        }
+        if (run - mn + 1 > kM2MaxSteps - 3) return 0;
+        worst = std::max(worst, kM2Unroll * ((run - mn + 1 + 3 + kM2Unroll - 1) / kM2Unroll));
+      }
+      return worst;
+    };
+    const size_t smem = march2_smem(p, W) + rr_smem_extra(v.ny);
+    const long key = ((long)MODE_RESID_RESTRICT * 32 + p.id) * 1024 + W;
+    auto it = m2_resident_.find(key);
+    if (it == m2_resident_.end()) {
+      int per_sm = 0;
+      CUDA_CHECK(cudaFuncSetAttribute(p.fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(march2_smem(p, kM2MaxW) + rr_smem_extra(2 * kM2MaxW))));
+      CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, p.fn, W, smem));
+      it = m2_resident_.emplace(key, std::max(1, per_sm) * sms_).first;
+    }
+    // (thread c reads the lists of the CTA's coarse row c: ncr <= W)
+    if (opt_.stencil_pair_rows > 0) {  // about as many fine rows per CTA as the residual kernel marches (2 ncr + 2)
+      int ncr = std::max(1, std::min(W, (std::min(kM2MaxSteps - 3, 6 * ((opt_.stencil_pair_rows + 3 + 5) / 6) - 3) - 2) / 2));
+      while (ncr > 0 && !max_steps(ncr)) --ncr;
+      return ncr;
+    }
+    // as march2_rows: minimise (waves of resident CTAs) x (row steps per CTA + prologue)
+    int best_ncr = 0;
+    double best = -1.0;
+    for (int ncr = 1; ncr <= std::min(W, kM2MaxSteps); ++ncr) {
+      const int steps = max_steps(ncr);
+      if (!steps) continue;
+      const double waves = std::ceil((double)((nxc + ncr - 1) / ncr) * B / std::max(1, it->second));
+      const double cost = waves * (steps + 5);
+      if (best < 0 || cost < best * 0.999) { best = cost; best_ncr = ncr; }
+    }
+    return best_ncr;
+  }
+  // bit l set: level l restricts its residual inside the residual kernel
+  int resid_restrict_levels() const {
+    int m = 0;
+    for (size_t l = 0; l < lv.size() && l < 31; ++l)
+      if (lv[l].rr_rows > 0) m |= 1 << l;
+    return m;
+  }
+  void resid_restrict(int l, const P *x, const P *rhs) {
+    if constexpr (std::is_same<P, float>::value && std::is_same<PC, float>::value) {
+      const Level &v = lv[l];
+      StencilArgs<P, PC> a;
+      a.nx = v.nx; a.ny = v.ny; a.x = x; a.rhs = rhs; a.y = nullptr;
+      a.fields = v.fields; a.field_bstride = v.fbstride; a.sigma = sigma_p_; a.cx = v.cx; a.cy = v.cy;
+      a.omega = opt_.mg_omega;
+      a.dinv = nullptr;
+      a.tr = v.tr_dev;
+      a.coarse = lv[l + 1].b;
+      const March2Pick p = resid_restrict_pick(v.ny);
+      int W = 0, nstrips = 0;
+      march2_strips(v.ny, W, nstrips);
+      dim3 grd(1, (v.tr.nxc + v.rr_rows - 1) / v.rr_rows, B);
+      p.fn<<<grd, W, march2_smem(p, W) + rr_smem_extra(v.ny), st_>>>(a, v.rr_rows);
+      if (l == 0) stats.stencil_applies++;
+      stats.launches++;
     }
   }
   template <typename TT, typename CC>
@@ -596,6 +719,7 @@ class BatchSolver {
                                                   : march2_rows(v.nx, nstrips, B, resident);
       dim3 grd(nstrips, (v.nx + rows - 1) / rows, B);
       p.fn<<<grd, W, march2_smem(p, W), st_>>>(a, rows);
+      last_m2_ = M2Launch{p.fn, grd, W, march2_smem(p, W), a, rows, stats.launches};
       return true;
     }
     return false;
@@ -735,6 +859,7 @@ class BatchSolver {
     if constexpr (kMixed) {
       convert_strided_kernel<T, P><<<cg, 256, 0, st_>>>(lenE, v, v_bs, lv[0].b, lenE);
       if (graph_exec_) {
+        if (graph_out_node_) set_graph_out(graph_result_);
         CUDA_CHECK(cudaGraphLaunch(graph_exec_, st_));
         stats.launches += graph_nodes_;
         stats.stencil_applies += graph_fine_applies_;
@@ -789,6 +914,7 @@ class BatchSolver {
       CUDA_CHECK(cudaStreamBeginCapture(st_, cudaStreamCaptureModeRelaxed));
       precondition_body(lv[0].b, nullptr, ncyc);
       cudaError_t e = cudaStreamEndCapture(st_, &graph);
+      const bool last_is_m2 = last_m2_.seq == stats.launches;
       graph_nodes_ = stats.launches - l0;
       graph_fine_applies_ = stats.stencil_applies - a0;
       stats.launches = l0;
@@ -802,12 +928,57 @@ class BatchSolver {
       if (cudaGraphInstantiate(&graph_exec_, graph, 0) != cudaSuccess) {
         cudaGetLastError();
         graph_exec_ = nullptr;
+        cudaGraphDestroy(graph);
+        return;
       }
-      cudaGraphDestroy(graph);
+      graph_ = graph;
+      // one V-cycle whose last kernel is a pair-kernel sweep writing graph_result_: that node can write the FGMRES Z slot itself
+      if (ncyc == 1 && last_is_m2 && static_cast<const void *>(last_m2_.a.y) == static_cast<const void *>(graph_result_)) {
+        size_t n = 0;
+        CUDA_CHECK(cudaGraphGetNodes(graph, nullptr, &n));
+        std::vector<cudaGraphNode_t> nodes(n);
+        CUDA_CHECK(cudaGraphGetNodes(graph, nodes.data(), &n));
+        cudaGraphNode_t leaf = nullptr;
+        int leaves = 0;
+        for (cudaGraphNode_t nd : nodes) {
+          size_t nd_out = 0;
+          CUDA_CHECK(cudaGraphNodeGetDependentNodes(nd, nullptr, &nd_out));
+          if (nd_out == 0) { leaf = nd; ++leaves; }
+        }
+        cudaGraphNodeType ty;
+        cudaKernelNodeParams kp;
+        if (leaves == 1 && cudaGraphNodeGetType(leaf, &ty) == cudaSuccess && ty == cudaGraphNodeTypeKernel &&
+            cudaGraphKernelNodeGetParams(leaf, &kp) == cudaSuccess && kp.func == reinterpret_cast<void *>(last_m2_.fn)) {
+          graph_out_node_ = leaf;
+          graph_out_launch_ = last_m2_;
+          graph_out_ = graph_result_;
+        }
+        cudaGetLastError();
+      }
+    }
+  }
+  // point the output of the graph's last sweep at y (graph_out_node_ only)
+  void set_graph_out(P *y) {
+    if constexpr (std::is_same<P, float>::value && std::is_same<PC, float>::value) {
+      if (y == graph_out_) return;
+      const M2Launch &l = graph_out_launch_;
+      StencilArgs<float, float> a = l.a;
+      int rows = l.rows;
+      a.y = y;
+      void *args[2] = {&a, &rows};
+      cudaKernelNodeParams kp = {};
+      kp.func = reinterpret_cast<void *>(l.fn);
+      kp.gridDim = l.grd;
+      kp.blockDim = dim3(l.W);
+      kp.sharedMemBytes = (unsigned)l.smem;
+      kp.kernelParams = args;
+      CUDA_CHECK(cudaGraphExecKernelNodeSetParams(graph_exec_, graph_out_node_, &kp));
+      graph_out_ = y;
     }
   }
   ~BatchSolver() {
     if (graph_exec_) cudaGraphExecDestroy(graph_exec_);
+    if (graph_) cudaGraphDestroy(graph_);
   }
 
   // Levels [fused_l0_, L) run as one kernel (csrc/coarse_kernel.cuh) when they fit in shared memory together: the
@@ -889,8 +1060,10 @@ class BatchSolver {
         std::swap(cur, oth);
       }
     }
-    apply(l, MODE_RESID, cur, rin, v.r);
-    {
+    if (v.rr_rows > 0) {
+      resid_restrict(l, cur, rin);  // lv[l + 1].b = R (rin - A cur), v.r is not written
+    } else {
+      apply(l, MODE_RESID, cur, rin, v.r);
       const TransferArgs &t = v.tr;
       dim3 blk(64, 4);
       if constexpr (sizeof(P) <= 8) {
@@ -907,11 +1080,12 @@ class BatchSolver {
         dim3 grd((t.nyc + 63) / 64, (t.nxc + 3) / 4, 2 * B);
         restrict_kernel<P><<<grd, blk, 0, st_>>>(t, v.r, lv[l + 1].b);
       }
-      stats.launches += 2;
+      stats.launches++;
     }
     vcycle(l + 1, lv[l + 1].b, nullptr);
     {
       const TransferArgs &t = v.tr;
+      stats.launches++;
       if (t.nyf >= 256 && opt_.transfer_tiled != 2) {  // four fine columns per thread
         dim3 blk(64, 4), grd((t.nyf + 255) / 256, (t.nxf + 3) / 4, 2 * B);
         if ((opt_.transfer_vec & 1) && std::is_same<P, float>::value && (t.nyf % 4) == 0) prolong_add4_kernel<P, true><<<grd, blk, 0, st_>>>(t, lv[l + 1].x, cur);
@@ -1293,14 +1467,18 @@ class BatchSolver {
       if (!input_staged) CUDA_CHECK(cudaMemcpyAsync(lv[0].b, v, vsE * sizeof(P), cudaMemcpyDeviceToDevice, st_));
       const int ncyc = mg_cycles_();
       if (graph_exec_) {
+        if (graph_out_node_) set_graph_out(z);  // the last sweep writes the Z slot
         CUDA_CHECK(cudaGraphLaunch(graph_exec_, st_));
         stats.launches += graph_nodes_;
         stats.stencil_applies += graph_fine_applies_;
+        if (!graph_out_node_) CUDA_CHECK(cudaMemcpyAsync(z, graph_result_, vsE * sizeof(P), cudaMemcpyDeviceToDevice, st_));
+      } else if (ncyc == 1) {
+        precondition_body(lv[0].b, z, 1);
       } else {
         precondition_body(lv[0].b, nullptr, ncyc);
-        graph_result_ = ncyc == 1 ? lv[0].x : pre_b_;
+        graph_result_ = pre_b_;
+        CUDA_CHECK(cudaMemcpyAsync(z, graph_result_, vsE * sizeof(P), cudaMemcpyDeviceToDevice, st_));
       }
-      CUDA_CHECK(cudaMemcpyAsync(z, graph_result_, vsE * sizeof(P), cudaMemcpyDeviceToDevice, st_));
     }
   }
 
@@ -1988,6 +2166,10 @@ class BatchSolver {
   std::map<long, int> m2_resident_;  // pair-marching kernel: resident CTAs on the device per (mode, prefetch depth, CTA width)
   cudaGraphExec_t graph_exec_ = nullptr;
   P *graph_result_ = nullptr;
+  cudaGraph_t graph_ = nullptr;
+  cudaGraphNode_t graph_out_node_ = nullptr;  // the graph's last sweep when it can be redirected (set_graph_out)
+  M2Launch graph_out_launch_;
+  P *graph_out_ = nullptr;                    // where that node writes now
   long graph_nodes_ = 0, graph_fine_applies_ = 0;
   cplx *ncomplex_ = nullptr, *fields_out_ = nullptr;
   double *jz_ = nullptr;
