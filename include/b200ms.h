@@ -29,7 +29,7 @@
 extern "C" {
 #endif
 
-#define B200MS_VERSION 206
+#define B200MS_VERSION 207
 
 /* return codes */
 enum {
@@ -195,6 +195,13 @@ typedef struct {
                             D = -1e18 f^2 (2 Re dn/df + f Re d2n/df2) / c0^2, c0 in um/s */
   double *d2n_residual;  /* NULL, or caller-allocated num_modes doubles: final relative residual of each mode's correction solve
                             (needs d2n_dfreq2) */
+  /* ---- since version 207: permittivity gradient of each mode's frequency derivative, from the correction solve of
+     d2n_dfreq2 (no further solve; see DESIGN.md §4).  Same scope as dn_dfreq; n_complex, the fields, dn_dfreq, dn_deps and
+     d2n_dfreq2 do not change when it is asked for ---- */
+  double *d2n_dfreq_deps; /* NULL, or caller-allocated 3*nx*ny*num_modes complex128 (re,im), layout of dn_deps: d(dn/df) / d eps_aa
+                            (1/Hz) of the caller's eps_cross at fixed d eps / df and PML stretch (0 at PEC-valued cells; NaN for a mode
+                            whose correction solve stopped above 100 x inner_tol).  Gradient of the group index for a real change of
+                            eps: Re dn_deps + f Re d2n_dfreq_deps.  HOST or DEVICE memory like `fields` */
 } b200ms_result;
 
 /* Tunables (all have defaults; see DESIGN.md). */

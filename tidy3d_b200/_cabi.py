@@ -17,7 +17,7 @@ import numpy as np
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("B200MS_LIB") or os.path.join(_HERE, "libb200ms.so")  # B200MS_LIB: developer override (A/B of builds)
 
-ABI_VERSION = 206  # B200MS_VERSION of include/b200ms.h
+ABI_VERSION = 207  # B200MS_VERSION of include/b200ms.h
 OK, ERR_SHAPE, ERR_NO_MODES, ERR_UNSUPPORTED, ERR_CUDA, ERR_NOCONV, ERR_ARG = range(7)
 SPEC_NAMES = {0: "diagonal", 1: "tensorial_real", 2: "tensorial_complex"}
 
@@ -47,7 +47,7 @@ class Result(C.Structure):
         ("fields", _dp), ("n_complex", _dp), ("flux", _dp), ("te_fraction", _dp), ("overlap_prev", _dp), ("eps_spec", C.c_int), ("status", C.c_int), ("converged", C.c_int),
         ("outer_iters", C.c_int), ("op_applies", C.c_int), ("inner_iters", C.c_int), ("stencil_applies", C.c_int),
         ("is_complex", C.c_int), ("solve_ms", C.c_double), ("total_ms", C.c_double), ("max_residual", C.c_double),
-        ("dn_dfreq", _dp), ("dn_deps", _dp), ("d2n_dfreq2", _dp), ("d2n_residual", _dp),
+        ("dn_dfreq", _dp), ("dn_deps", _dp), ("d2n_dfreq2", _dp), ("d2n_residual", _dp), ("d2n_dfreq_deps", _dp),
     ]  # fmt: skip
 
 
@@ -336,20 +336,21 @@ class Handle:
             pass
 
     def solve_batch(self, packed, want_fields=True, fields_ptrs=None, want_flux=False, want_overlaps=False, want_dfreq=False, want_deps=False,
-                    want_d2freq=False):
+                    want_d2freq=False, want_group_eps=False):
         """packed: list of PackedProblem.  Returns (rc, fields list | None, n_complex list, Result structs).
 
         ``fields_ptrs``: optional list of raw addresses (host or DEVICE memory, e.g. ``tensor.data_ptr()``) the library
         writes the fields of each problem to, instead of freshly allocated pinned host arrays; then ``fields`` is None.
         Fields are complex128, or complex64 for ``precision == "single"`` problems (solver.py:265-267).  ``want_dfreq`` /
         ``want_deps``: d n / df and d n / d eps of every mode (``last_dn_dfreq`` / ``last_dn_deps``); ``want_d2freq``: d^2 n / df^2 and
-        the residual of its correction solve (``last_d2n_dfreq2`` / ``last_d2n_residual``)."""
+        the residual of its correction solve (``last_d2n_dfreq2`` / ``last_d2n_residual``); ``want_group_eps``: d(dn/df) / d eps of
+        every mode from that correction solve (``last_d2n_dfreq_deps``)."""
         n = len(packed)
         probs = (Problem * n)(*[p.struct for p in packed])
         results = (Result * n)()
         fields, ncs = [], []
         self.last_flux, self.last_te, self.last_overlaps, self.last_dn_dfreq, self.last_dn_deps = [], [], [], [], []
-        self.last_d2n_dfreq2, self.last_d2n_residual = [], []
+        self.last_d2n_dfreq2, self.last_d2n_residual, self.last_d2n_dfreq_deps = [], [], []
         for i, p in enumerate(packed):
             nc = np.zeros(p.num_modes, dtype=np.complex128)
             ncs.append(nc)
@@ -368,6 +369,10 @@ class Handle:
                 self.last_d2n_residual.append(r)
                 results[i].d2n_dfreq2 = _ptr(d.view(np.float64))
                 results[i].d2n_residual = _ptr(r)
+            if want_group_eps:
+                d = np.zeros((3, p.nx, p.ny, p.num_modes), dtype=np.complex128)
+                self.last_d2n_dfreq_deps.append(d)
+                results[i].d2n_dfreq_deps = _ptr(d.view(np.float64))
             if want_flux:
                 fl, te = np.zeros(p.num_modes), np.zeros(p.num_modes)
                 self.last_flux.append(fl)

@@ -869,7 +869,8 @@ void derivative_pass(b200ms_handle *h, BatchSolver<T, C, P, PC> &S, const std::v
 // Dispersion pass of one device batch (csrc/derivatives.cuh), after derivative_pass (whose device tables `da` it reads):
 // result.d2n_dfreq2 and result.d2n_residual of the problems that ask for them.  Per mode slot q: the projected right-hand side
 // r = -Pi A'v, one correction solve (A - lambda_q) x = r by the eigen-solve's own inner solver (Krylov shift lambda_q of every
-// problem; the multigrid stays built for sigma) and a scan for w^T A'x.  It writes its own buffers, the first two slots of the
+// problem; the multigrid stays built for sigma) and a scan for w^T A'x.  With result.d2n_dfreq_deps, group_grad_kernel then
+// sums w_hat^T v and writes slot q of the map from the same x.  It writes its own buffers, the first two slots of the
 // outer Krylov basis and the inner solver's scratch -- nothing the fields, the post-processing or the warm start read.
 template <typename T, typename C, typename P, typename PC>
 void dispersion_pass(b200ms_handle *h, BatchSolver<T, C, P, PC> &S, const std::vector<const ProblemSetup *> &ps, const std::vector<int> &ids,
@@ -878,10 +879,12 @@ void dispersion_pass(b200ms_handle *h, BatchSolver<T, C, P, PC> &S, const std::v
   const int B = (int)ids.size(), k = S.k, nx = S.nx, ny = S.ny;
   const size_t N = (size_t)nx * ny;
   std::vector<char> skip(B);
-  bool any_mat = false;
+  bool any_mat = false, any_gmap = false;
   for (int b = 0; b < B; ++b) {
     const b200ms_problem &p = prob[W.i0 + ids[b]];
-    skip[b] = res[W.i0 + ids[b]].d2n_dfreq2 ? 0 : 1;
+    const b200ms_result &rb = res[W.i0 + ids[b]];
+    skip[b] = (rb.d2n_dfreq2 || rb.d2n_dfreq_deps) ? 0 : 1;
+    any_gmap = any_gmap || rb.d2n_dfreq_deps;
     any_mat = any_mat || (p.eps ? (p.eps_dfreq || p.eps_d2freq) : (p.section->deps_table || p.section->d2eps_table));
   }
   // host tables: f^2 d^2c/df^2 = 2 (f dc/df)^2 / c = 2 c (kappa / s)^2, frequencies
@@ -914,7 +917,10 @@ void dispersion_pass(b200ms_handle *h, BatchSolver<T, C, P, PC> &S, const std::v
   const size_t o_beta = o_sum + align256((size_t)B * 3 * sizeof(cplx)), o_p1 = o_beta + align256(B * sizeof(cplx));
   const size_t pbytes = any_mat ? align256((size_t)B * 3 * N * sizeof(cplx)) : 0, o_p2 = o_p1 + pbytes, o_sec = o_p2 + pbytes;
   const size_t sec_bytes = any_mat ? std::max(gather_scratch_bytes(ids, W, prob, nx, ny, tab1), gather_scratch_bytes(ids, W, prob, nx, ny, tab2)) : 0;
-  h->disp.reserve(o_sec + sec_bytes + 256);
+  // group-gradient pass: per-problem (alpha, beta), the sum w_hat^T v and the map [B][3][N][M]
+  const size_t o_ab = align256(o_sec + sec_bytes), o_hsum = o_ab + align256((size_t)B * 2 * sizeof(cplx));
+  const size_t o_gmap = o_hsum + align256((size_t)B * 3 * sizeof(cplx));
+  h->disp.reserve(any_gmap ? o_gmap + (size_t)B * 3 * N * k * sizeof(cplx) + 256 : o_sec + sec_bytes + 256);
   unsigned char *base = h->disp.p;
   cudaStream_t st = h->stream;
   CUDA_CHECK(cudaMemcpyAsync(base + o_c2x, c2x.data(), c2x.size() * sizeof(T), cudaMemcpyHostToDevice, st));
@@ -979,7 +985,7 @@ void dispersion_pass(b200ms_handle *h, BatchSolver<T, C, P, PC> &S, const std::v
     scan(2, sx);  // w^T x, w^T A'x
     for (int b = 0; b < B; ++b) {
       b200ms_result &rr = res[W.i0 + ids[b]];
-      if (skip[b]) continue;
+      if (skip[b] || !rr.d2n_dfreq2) continue;
       const cplx *s = sv.data() + (size_t)b * 3, *t = sx.data() + (size_t)b * 3;
       const cd wv(s[0].re, s[0].im), l1 = cd(s[1].re, s[1].im) / wv, a2(s[2].re, s[2].im);
       const cd wx(t[0].re, t[0].im), w1x(t[1].re, t[1].im);
@@ -994,8 +1000,45 @@ void dispersion_pass(b200ms_handle *h, BatchSolver<T, C, P, PC> &S, const std::v
       rr.d2n_dfreq2[2 * q + 1] = d2n.imag();
       if (rr.d2n_residual) rr.d2n_residual[q] = resv[b];
     }
+    if (any_gmap) {  // d_g (dn/df) of slot q while x still holds its correction
+      const dim3 g0(nch, B);
+      cplx *hsum = reinterpret_cast<cplx *>(base + o_hsum), *dab = reinterpret_cast<cplx *>(base + o_ab);
+      cplx *gmap = reinterpret_cast<cplx *>(base + o_gmap);
+      if (S.has_mu) group_grad_kernel<T, C, true><<<g0, 256, 0, st>>>(a, 0, dab, gmap);
+      else group_grad_kernel<T, C, false><<<g0, 256, 0, st>>>(a, 0, dab, gmap);
+      deriv_final_kernel<<<(B * 3 + 127) / 128, 128, 0, st>>>(a.partial, nch, B * 3, hsum);
+      CUDA_CHECK(cudaGetLastError());
+      std::vector<cplx> sh((size_t)B * 3), ab((size_t)B * 2);
+      CUDA_CHECK(cudaMemcpyAsync(sh.data(), hsum, sh.size() * sizeof(cplx), cudaMemcpyDeviceToHost, st));
+      CUDA_CHECK(cudaStreamSynchronize(st));
+      // map = alpha (chi E + chi' D) + beta chi D:  d_g (dn/df) = knorm [-d_g lambda' / (2 s f) - (lambda' / f) d_g lambda / (4 s^3)]
+      for (int b = 0; b < B; ++b) {
+        const cplx *s = sv.data() + (size_t)b * 3, *t = sx.data() + (size_t)b * 3;
+        const cd wv(s[0].re, s[0].im), l1 = cd(s[1].re, s[1].im) / wv, wx(t[0].re, t[0].im), hv(sh[(size_t)b * 3].re, sh[(size_t)b * 3].im);
+        const double f = freq[b], kn = ps[b]->knorm;
+        const cd sn = nsorted[(size_t)b * k + q];
+        cd al = -kn / (2.0 * sn * f * wv), be = -al * (hv + wx) / wv - kn * l1 / (4.0 * f * sn * sn * sn * wv);
+        if (skip[b] || std::abs(wv) == 0 || !(resv[b] <= 100.0 * tol)) al = be = cd(std::nan(""), std::nan(""));
+        ab[2 * b] = mk(al.real(), al.imag());
+        ab[2 * b + 1] = mk(be.real(), be.imag());
+      }
+      CUDA_CHECK(cudaMemcpyAsync(dab, ab.data(), ab.size() * sizeof(cplx), cudaMemcpyHostToDevice, st));
+      const dim3 blk(64, 4), grd((ny + 63) / 64, (nx + 3) / 4, B);
+      if (S.has_mu) group_grad_kernel<T, C, true><<<grd, blk, 0, st>>>(a, 1, dab, gmap);
+      else group_grad_kernel<T, C, false><<<grd, blk, 0, st>>>(a, 1, dab, gmap);
+      CUDA_CHECK(cudaGetLastError());
+      h->stats.launches += 3;
+    }
   }
   S.reset_sigma();
+  if (!any_gmap) return;
+  const cplx *gmap = reinterpret_cast<const cplx *>(base + o_gmap);
+  for (int b = 0; b < B; ++b) {
+    b200ms_result &r = res[W.i0 + ids[b]];
+    if (r.d2n_dfreq_deps)
+      CUDA_CHECK(cudaMemcpyAsync(r.d2n_dfreq_deps, gmap + (size_t)b * 3 * N * k, 3 * N * k * sizeof(cplx), cudaMemcpyDefault, st));
+  }
+  CUDA_CHECK(cudaStreamSynchronize(st));
 }
 
 template <typename T, typename C, typename P, typename PC>
@@ -1098,8 +1141,8 @@ void solve_group(b200ms_handle *h, const std::vector<int> &ids, const Window &W,
   bool want_deriv = false, want_disp = false;
   for (int b = 0; b < B; ++b) {
     const b200ms_result &rb = res[W.i0 + ids[b]];
-    want_deriv = want_deriv || rb.dn_dfreq || rb.dn_deps || rb.d2n_dfreq2;
-    want_disp = want_disp || rb.d2n_dfreq2;
+    want_deriv = want_deriv || rb.dn_dfreq || rb.dn_deps || rb.d2n_dfreq2 || rb.d2n_dfreq_deps;
+    want_disp = want_disp || rb.d2n_dfreq2 || rb.d2n_dfreq_deps;
   }
   if (want_deriv) {
     DerivArgs<T, C> da;
@@ -1240,7 +1283,7 @@ extern "C" int b200ms_solve_batch(b200ms_handle *h, int nprob, const b200ms_prob
           res[i].eps_spec = s.eps_spec;
           res[i].is_complex = s.is_complex;
           std::string err = s.error;
-          if (res[i].status == B200MS_OK && (res[i].dn_dfreq || res[i].dn_deps || res[i].d2n_dfreq2) && (s.tensorial || s.relative || s.masked)) {
+          if (res[i].status == B200MS_OK && (res[i].dn_dfreq || res[i].dn_deps || res[i].d2n_dfreq2 || res[i].d2n_dfreq_deps) && (s.tensorial || s.relative || s.masked)) {
             res[i].status = B200MS_ERR_UNSUPPORTED;
             err = s.tensorial ? "mode derivatives: tensorial problems (angled planes, off-diagonal eps) are not supported"
                   : s.relative ? "mode derivatives: the relative mode solver (basis fields) is not supported"

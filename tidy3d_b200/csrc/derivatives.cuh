@@ -341,4 +341,194 @@ __global__ void disp_fields_kernel(int nx, int ny, int B, const C *fields, size_
   }
 }
 
+// ------------------------------------------------------------------------------------------------
+// Group-gradient pass: d_g (dn/df), the permittivity gradient of each mode's frequency derivative, from the dispersion pass's
+// correction x (oracle/mode_group_gradient.py is the float64 model).  With p = (exx, eyy, iez) of the solver frame,
+// D_a(w, e) = w^T (dA/dp_a(g)) e is a local product, quadratic in the 1-D coefficients and affine in p, and
+//   d_g lambda' w^T v = chi_a [D_a(w_hat, v) + D_a(w, x) + D_a'(w, v)] + chi_a' D_a(w, v) - chi_a D_a(w, v) (w_hat^T v + w^T x) / w^T v
+// with w_hat = G'J Q v + G J Q'v + G J Q x (l' = -i Im l for every stretched length), chi = (1/je, 1/je, -iez^2 je),
+// chi' = (0, 0, -2 iez iez' je).  Mode 0 sums w_hat^T v per chunk; mode 1 writes
+//   map[b][a][g][q] = alpha_b (chi_a E_a + chi_a' D_a) + beta_b chi_a D_a,   E_a = D_a(w_hat, v) + D_a(w, x) + D_a'(w, v),
+// with alpha, beta the per-problem scalars of dispersion_pass (NaN for a correction solve that stopped above 100 x inner_tol).
+// ------------------------------------------------------------------------------------------------
+
+template <typename T, typename C, bool HAS_MU>
+struct GroupCell {
+  const T *v, *x;          // this slot's Ritz vector and correction, [e1 | e2]
+  const C *fb;             // this problem's coefficient fields: exx, eyy, iez, mxx, myy, imz at fb + k N
+  const T *cx, *cy, *dcx, *dcy;  // [4][n] 1-D coefficients and f dc/df
+  const cplx *gx, *gy;     // [2][n] primal / dual stretched lengths
+  const cplx *p1;          // [3][N] f dp/df, or null
+  int nx, ny;
+  size_t N;
+  __device__ __forceinline__ bool in(int ii, int jj) const { return ii >= 0 && ii < nx && jj >= 0 && jj < ny; }
+  __device__ __forceinline__ cplx ld(const T *e, int ii, int jj) const { return in(ii, jj) ? to_cplx(ldg(e + (size_t)ii * ny + jj)) : mk(0.0, 0.0); }
+  __device__ __forceinline__ cplx co(const T *c, int n, int w, int i) const { return (i >= 0 && i < n) ? to_cplx(ldg(c + (size_t)w * n + i)) : mk(0.0, 0.0); }
+  // 1-D coefficient w of x (ax 0) or y (ax 1) at c + sc c'
+  __device__ __forceinline__ cplx cc(int ax, int w, int i, double sc) const {
+    cplx c = ax == 0 ? co(cx, nx, w, i) : co(cy, ny, w, i);
+    if (sc != 0.0) c += sc * (ax == 0 ? co(dcx, nx, w, i) : co(dcy, ny, w, i));
+    return c;
+  }
+  // coefficient field k (exx, eyy, iez) at (ii, jj) moved by sp p' (zero outside the grid)
+  __device__ __forceinline__ cplx fld(int k, int ii, int jj, double sp) const {
+    if (!in(ii, jj)) return mk(0.0, 0.0);
+    const size_t g = (size_t)ii * ny + jj;
+    cplx e = to_cplx(ldg(fb + (size_t)k * N + g));
+    if (p1 && sp != 0.0) e += sp * ldg(p1 + (size_t)k * N + g);
+    return e;
+  }
+  __device__ __forceinline__ cplx imz(int ii, int jj) const { return HAS_MU ? to_cplx(ldg(fb + 5 * N + (size_t)ii * ny + jj)) : mk(1.0, 0.0); }
+  // t = imz (Dxf e2 - Dyf e1) at (ii, jj) and, with D, its coefficient derivative dt
+  template <bool D>
+  __device__ __forceinline__ void tt(const T *e, int ii, int jj, cplx &t, cplx &dt) const {
+    t = dt = mk(0.0, 0.0);
+    if (!in(ii, jj)) return;
+    const cplx a2 = ld(e + N, ii, jj), b2 = ld(e + N, ii + 1, jj), a1 = ld(e, ii, jj), b1 = ld(e, ii, jj + 1);
+    const cplx mz = imz(ii, jj);
+    t = mz * (co(cx, nx, 0, ii) * a2 + co(cx, nx, 1, ii) * b2 - co(cy, ny, 0, jj) * a1 - co(cy, ny, 1, jj) * b1);
+    if (D) dt = mz * (co(dcx, nx, 0, ii) * a2 + co(dcx, nx, 1, ii) * b2 - co(dcy, ny, 0, jj) * a1 - co(dcy, ny, 1, jj) * b1);
+  }
+  // w = G J Q v and w_hat = G'J Q v + G J (Q'v + Q x) at (ii, jj); zero outside the grid
+  __device__ __forceinline__ void ww(int ii, int jj, cplx w[2], cplx h[2]) const {
+    w[0] = w[1] = h[0] = h[1] = mk(0.0, 0.0);
+    if (!in(ii, jj)) return;
+    cplx t0, d0, tm, dm, tn, dn, u;
+    tt<true>(v, ii, jj, t0, d0);
+    tt<true>(v, ii - 1, jj, tm, dm);
+    tt<true>(v, ii, jj - 1, tn, dn);
+    const cplx e1 = ld(v, ii, jj), e2 = ld(v + N, ii, jj), ex = fld(0, ii, jj, 0.0), ey = fld(1, ii, jj, 0.0);
+    const cplx cx2 = co(cx, nx, 2, ii), cx3 = co(cx, nx, 3, ii), cy2 = co(cy, ny, 2, jj), cy3 = co(cy, ny, 3, jj);
+    const cplx q1 = cx2 * t0 + cx3 * tm + ey * e2, q2 = cy2 * t0 + cy3 * tn - ex * e1;
+    cplx dq1 = co(dcx, nx, 2, ii) * t0 + cx2 * d0 + co(dcx, nx, 3, ii) * tm + cx3 * dm;
+    cplx dq2 = co(dcy, ny, 2, jj) * t0 + cy2 * d0 + co(dcy, ny, 3, jj) * tn + cy3 * dn;
+    if (p1) {
+      const size_t g = (size_t)ii * ny + jj;
+      dq1 += ldg(p1 + N + g) * e2;
+      dq2 -= ldg(p1 + g) * e1;
+    }
+    tt<false>(x, ii, jj, t0, u);
+    tt<false>(x, ii - 1, jj, tm, u);
+    tt<false>(x, ii, jj - 1, tn, u);
+    dq1 += cx2 * t0 + cx3 * tm + ey * ld(x + N, ii, jj);
+    dq2 += cy2 * t0 + cy3 * tn - ex * ld(x, ii, jj);
+    const cplx lfx = gx[ii], lbx = gx[nx + ii], lfy = gy[jj], lby = gy[ny + jj];
+    const cplx Gf = lfx * lby, Gb = lbx * lfy;
+    const cplx dGf = mk(0.0, -lfx.im) * lby + lfx * mk(0.0, -lby.im), dGb = mk(0.0, -lbx.im) * lfy + lbx * mk(0.0, -lfy.im);
+    w[0] = Gf * q2;
+    w[1] = -(Gb * q1);
+    h[0] = dGf * q2 + Gf * dq2;
+    h[1] = -(dGb * q1 + Gb * dq1);
+  }
+  // D_a(W, e) at (i, j) with coefficients c + sc c' and fields p + sp p'; W: w at (i,j), (i-1,j), (i,j-1), (i+1,j), (i+1,j-1),
+  // (i,j+1), (i-1,j+1)
+  __device__ __forceinline__ void forms(int i, int j, const cplx (&W)[7][2], const T *e, double sc, double sp, cplx d[3]) const {
+    cplx z[3] = {mk(0.0, 0.0), mk(0.0, 0.0), mk(0.0, 0.0)};
+#pragma unroll
+    for (int s = 0; s < 7; ++s) zadd(s, i, j, W[s][0], W[s][1], sc, z);
+    forms_z(i, j, z, W[0][0], W[0][1], e, sc, sp, d);
+  }
+  // z = Dxf^T w1 + Dyf^T w2 at (i, j), (i+1, j), (i, j+1) with coefficients c + sc c': the part of stencil site s (numbered as
+  // for forms) holding w = (w1, w2)
+  __device__ __forceinline__ void zadd(int s, int i, int j, cplx w1, cplx w2, double sc, cplx z[3]) const {
+    switch (s) {
+      case 0:
+        z[0] += cc(0, 0, i, sc) * w1 + cc(1, 0, j, sc) * w2;
+        if (in(i + 1, j)) z[1] += cc(0, 1, i, sc) * w1;
+        if (in(i, j + 1)) z[2] += cc(1, 1, j, sc) * w2;
+        break;
+      case 1: z[0] += cc(0, 1, i - 1, sc) * w1; break;
+      case 2: z[0] += cc(1, 1, j - 1, sc) * w2; break;
+      case 3: z[1] += cc(0, 0, i + 1, sc) * w1 + cc(1, 0, j, sc) * w2; break;
+      case 4: z[1] += cc(1, 1, j - 1, sc) * w2; break;
+      case 5: z[2] += cc(0, 0, i, sc) * w1 + cc(1, 0, j + 1, sc) * w2; break;
+      default: z[2] += cc(0, 1, i - 1, sc) * w1; break;
+    }
+  }
+  // D_a from z at (i, j), (i+1, j), (i, j+1) and w at (i, j)
+  __device__ __forceinline__ void forms_z(int i, int j, const cplx z[3], cplx w01, cplx w02, const T *e, double sc, double sp, cplx d[3]) const {
+    const size_t g = (size_t)i * ny + j;
+    const cplx zg = z[0], zx = z[1], zy = z[2];
+    const cplx e1 = ld(e, i, j), e2 = ld(e + N, i, j), iz = fld(2, i, j, sp);
+    const cplx mx = HAS_MU ? to_cplx(ldg(fb + 3 * N + g)) : mk(1.0, 0.0), my = HAS_MU ? to_cplx(ldg(fb + 4 * N + g)) : mk(1.0, 0.0);
+    d[0] = -(e1 * (cc(0, 2, i, sc) * iz * zg + cc(0, 3, i + 1, sc) * fld(2, i + 1, j, sp) * zx + my * w01));
+    d[1] = -(e2 * (cc(1, 2, j, sc) * iz * zg + cc(1, 3, j + 1, sc) * fld(2, i, j + 1, sp) * zy + mx * w02));
+    const cplx s = cc(0, 2, i, sc) * (fld(0, i, j, sp) * e1) + cc(0, 3, i, sc) * (fld(0, i - 1, j, sp) * ld(e, i - 1, j)) +
+                   cc(1, 2, j, sc) * (fld(1, i, j, sp) * e2) + cc(1, 3, j, sc) * (fld(1, i, j - 1, sp) * ld(e + N, i, j - 1));
+    d[2] = -(zg * s);
+  }
+};
+
+// grid (nchunk, B) x 256 threads (mode 0) or like deriv_map_kernel for one mode slot (mode 1), see above.  ab: [B][2] (alpha,
+// beta); map: [B][3][N][M].
+template <typename T, typename C, bool HAS_MU>
+__global__ void __launch_bounds__(256) group_grad_kernel(DispArgs<T, C> a, int mode, const cplx *ab, cplx *map) {
+  const DerivArgs<T, C> &d = a.d;
+  const int nx = d.nx, ny = d.ny, M = d.num_modes;
+  const size_t N = (size_t)nx * ny;
+  const int b = mode == 0 ? blockIdx.y : blockIdx.z;
+  const T *vb = d.vec + (size_t)a.q * d.vstride + (size_t)b * 2 * N;
+  const GroupCell<T, C, HAS_MU> G{vb, a.x + (size_t)b * 2 * N, d.fields + d.field_bstride * b,
+                                  d.cx + (size_t)b * 4 * nx, d.cy + (size_t)b * 4 * ny, d.dcx + (size_t)b * 4 * nx, d.dcy + (size_t)b * 4 * ny,
+                                  d.gx + (size_t)b * 2 * nx, d.gy + (size_t)b * 2 * ny, a.p1 ? a.p1 + (size_t)b * 3 * N : nullptr, nx, ny, N};
+  if (mode == 0) {
+    cplx s = mk(0.0, 0.0);
+    for (size_t g = (size_t)blockIdx.x * 256 + threadIdx.x; g < N; g += (size_t)gridDim.x * 256) {
+      const int i = (int)(g / ny), j = (int)(g % ny);
+      cplx w[2], h[2];
+      G.ww(i, j, w, h);
+      s += h[0] * G.ld(vb, i, j) + h[1] * G.ld(vb + N, i, j);
+    }
+    __shared__ cplx red[256];
+    red[threadIdx.x] = s;
+    __syncthreads();
+    for (int hh = 128; hh > 0; hh >>= 1) {
+      if ((int)threadIdx.x < hh) red[threadIdx.x] += red[threadIdx.x + hh];
+      __syncthreads();
+    }
+    if (threadIdx.x < 3) a.partial[((size_t)b * gridDim.x + blockIdx.x) * 3 + threadIdx.x] = threadIdx.x == 0 ? red[0] : mk(0.0, 0.0);
+    return;
+  }
+  const int j = blockIdx.x * 64 + threadIdx.x, i = blockIdx.y * 4 + threadIdx.y;
+  if (i >= nx || j >= ny) return;
+  const int di[7] = {0, -1, 0, 1, 1, 0, -1}, dj[7] = {0, 0, -1, 0, -1, 1, 1};
+  // D_a(w_hat, v) streams over the stencil (only z and w_hat(i, j) are kept); then the w stencil is kept for the other forms
+  cplx W[7][2], un[2], hz[3] = {mk(0.0, 0.0), mk(0.0, 0.0), mk(0.0, 0.0)}, h0[2];
+#pragma unroll
+  for (int s = 0; s < 7; ++s) {
+    cplx hs[2];
+    G.ww(i + di[s], j + dj[s], un, hs);
+    G.zadd(s, i, j, hs[0], hs[1], 0.0, hz);
+    if (s == 0) h0[0] = hs[0], h0[1] = hs[1];
+  }
+  cplx d0[3], e[3], t[3];
+  G.forms_z(i, j, hz, h0[0], h0[1], vb, 0.0, 0.0, e);
+#pragma unroll
+  for (int s = 0; s < 7; ++s) G.ww(i + di[s], j + dj[s], W[s], un);
+  G.forms(i, j, W, vb, 0.0, 0.0, d0);
+  G.forms(i, j, W, G.x, 0.0, 0.0, t);
+  for (int k = 0; k < 3; ++k) e[k] += t[k];
+#pragma unroll 1
+  for (int s = 0; s < (a.p1 ? 4 : 2); ++s) {  // D_a'(w, v): +-c', then +-p'
+    const double st = (s & 1) ? -0.5 : 0.5;
+    G.forms(i, j, W, vb, s < 2 ? 2.0 * st : 0.0, s < 2 ? 0.0 : 2.0 * st, t);
+    for (int k = 0; k < 3; ++k) e[k] += st * t[k];
+  }
+  const size_t g = (size_t)i * ny + j;
+  const cplx iz = to_cplx(ldg(G.fb + 2 * N + g));
+  const double je = d.jz_e ? d.jz_e[(size_t)b * d.jz_len + (d.jz_axis == 0 ? i : j)] : 1.0;
+  const cplx chi[3] = {mk(1.0 / je, 0.0), mk(1.0 / je, 0.0), -(iz * iz) * je};
+  const cplx chi1 = a.p1 ? -2.0 * je * (iz * ldg(a.p1 + (size_t)b * 3 * N + 2 * N + g)) : mk(0.0, 0.0);
+  const cplx al = ab[2 * b], be = ab[2 * b + 1];
+  const double pec = 0.9 * 1e8;  // PEC-valued input, as eps_grad
+  const bool is_pec[3] = {abs2(to_cplx(ldg(G.fb + g))) >= pec * pec, abs2(to_cplx(ldg(G.fb + N + g))) >= pec * pec, abs2(iz) * pec * pec <= 1.0};
+  cplx *o = map + (size_t)b * 3 * N * M;
+  for (int k = 0; k < 3; ++k) {
+    cplx num = chi[k] * e[k], g0 = chi[k] * d0[k];
+    if (k == 2) num += chi1 * d0[k];
+    if (is_pec[k]) num = g0 = mk(0.0, 0.0);
+    o[((size_t)k * N + g) * M + a.q] = al * num + be * g0;
+  }
+}
+
 }  // namespace b200ms

@@ -109,16 +109,23 @@ def compute_modes_batch(
     correction solve stopped above 100 x the inner tolerance), ``d2n_residual`` (that solve's final relative residual) and
     ``dispersion`` (ps/(nm km), ``plugin.dispersion_of``: the step -> 0 limit of ``plugin.group_index``), and implies
     ``"freq"``; its material term comes from a problem's ``eps_dfreq=`` and ``eps_d2freq=`` (d^2 eps_cross / df^2) or a
-    section's callable media.  ``n_complex``, the fields, ``dn_dfreq`` and ``dn_deps`` do not change.
+    section's callable media.  ``n_complex``, the fields, ``dn_dfreq`` and ``dn_deps`` do not change.  ``"group_eps"`` adds the
+    permittivity gradient of the group index from the same correction solves (no further solve): ``d2n_dfreq_deps`` (3, Nx, Ny, M),
+    d(dn/df) / d eps_{xx,yy,zz} (1/Hz) at every Yee site at fixed d eps / df and PML stretch (NaN where ``d2n_dfreq2`` is), and
+    ``dng_deps`` = Re ``dn_deps`` + f Re ``d2n_dfreq_deps``, the gradient of ``n_group`` for a real change of eps.  It implies
+    ``"freq"``, ``"eps"`` and ``"freq2"``, whose outputs do not change.
     """
     post = tuple(post or ())
     unknown = set(post) - {"gauge", "normalize", "flux", "overlaps"}
     if unknown:
         raise ValueError(f"unknown post-processing step(s): {sorted(unknown)}")
     derivatives = tuple(derivatives or ())
-    unknown = set(derivatives) - {"freq", "eps", "freq2"}
+    unknown = set(derivatives) - {"freq", "eps", "freq2", "group_eps"}
     if unknown:
         raise ValueError(f"unknown derivative(s): {sorted(unknown)}")
+    group_eps = "group_eps" in derivatives
+    if group_eps:
+        derivatives = derivatives + tuple(d for d in ("eps", "freq2") if d not in derivatives)
     second = "freq2" in derivatives
     if second and "freq" not in derivatives:
         derivatives = derivatives + ("freq",)
@@ -159,12 +166,13 @@ def compute_modes_batch(
         packed.append(pk)
     h = handle or get_handle(device)  # after input validation: argument errors do not need a GPU
     with h.lock:
-        dkw = dict(want_dfreq="freq" in derivatives, want_deps="eps" in derivatives, want_d2freq=second) if derivatives else {}
+        dkw = dict(want_dfreq="freq" in derivatives, want_deps="eps" in derivatives, want_d2freq=second, want_group_eps=group_eps) if derivatives else {}
         rc, fields, ncs, results = h.solve_batch(packed, want_fields, fields_ptrs, want_flux=("flux" in post or "normalize" in post),
                                                  want_overlaps="overlaps" in post, **dkw)
         flux_out, te_out, ov_out = h.last_flux, h.last_te, h.last_overlaps
         dfreq_out, deps_out = (h.last_dn_dfreq, h.last_dn_deps) if derivatives else ([], [])
         d2_out, d2res_out = (h.last_d2n_dfreq2, h.last_d2n_residual) if second else ([], [])
+        gmap_out = h.last_d2n_dfreq_deps if group_eps else []
         err = h.last_error() if rc != _cabi.OK else ""
     if rc != _cabi.OK:
         bad = [i for i in range(len(packed)) if results[i].status != _cabi.OK]
@@ -197,6 +205,9 @@ def compute_modes_batch(
             infos[-1]["d2n_dfreq2"] = d2_out[i]
             infos[-1]["d2n_residual"] = d2res_out[i]
             infos[-1]["dispersion"] = dispersion_of(float(packed[i].struct.freq), dfreq_out[i], d2_out[i])
+        if gmap_out:
+            infos[-1]["d2n_dfreq_deps"] = gmap_out[i]
+            infos[-1]["dng_deps"] = deps_out[i].real + float(packed[i].struct.freq) * gmap_out[i].real
     return (out, infos) if return_info else out
 
 

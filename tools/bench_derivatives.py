@@ -2,9 +2,11 @@
   plain        -- one solve per frequency, no derivatives;
   analytic     -- one solve per frequency with derivatives=("freq",) (n_group from the left eigenvector);
   analytic_gvd -- one solve per frequency with derivatives=("freq2",) (n_group and the dispersion, one correction solve per mode);
+  gvd_eps      -- derivatives=("eps", "freq2"): the dispersion pass plus the first-order permittivity map;
+  group_eps    -- derivatives=("group_eps",): the same plus the group-index gradient map from the same correction solves;
   fd3          -- three solves per frequency at f(1 -/+ step) and f, n_group and dispersion by plugin.group_index (the reference's path).
 Prints one JSON line: solves/s, frequencies-with-group-index/s, frequencies-with-dispersion/s, the device time the derivative
-and dispersion passes add per problem, the correction solves' inner iterations per mode, the largest differences against fd3 and
+and dispersion passes add per problem, the time the group-index gradient map adds per problem (group_eps - gvd_eps), the correction solves' inner iterations per mode, the largest differences against fd3 and
 the derivative pass's algorithmic bytes against the 3.35 TB/s HBM3 data-sheet figure, with the card name and power limit read
 in the same run.
 
@@ -59,6 +61,8 @@ def main():
         "plain": lambda: compute_modes_batch(probs(wl.freqs), handle=h, want_fields=False, return_info=True),
         "analytic": lambda: compute_modes_batch(probs(wl.freqs), handle=h, want_fields=False, return_info=True, derivatives=("freq",)),
         "analytic_gvd": lambda: compute_modes_batch(probs(wl.freqs), handle=h, want_fields=False, return_info=True, derivatives=("freq2",)),
+        "gvd_eps": lambda: compute_modes_batch(probs(wl.freqs), handle=h, want_fields=False, return_info=True, derivatives=("eps", "freq2")),
+        "group_eps": lambda: compute_modes_batch(probs(wl.freqs), handle=h, want_fields=False, return_info=True, derivatives=("group_eps",)),
         "fd3": lambda: compute_modes_batch(probs(f3), handle=h, want_fields=False, return_info=True),
     }
     for fn in arms.values():  # warm-up of every shape
@@ -81,15 +85,18 @@ def main():
             if k == "analytic_gvd":
                 disp["analytic_gvd"] = np.array([i["dispersion"] for i in infos])
                 res_gvd = np.array([i["d2n_residual"] for i in infos])
+            if k == "group_eps":
+                gmap_finite = all(np.isfinite(i["d2n_dfreq_deps"]).all() for i in infos)
             if k == "fd3":
                 _, _, ng["fd3"], disp["fd3"] = plugin.group_index(np.array([o[1] for o in out]), f3, a.step)
-    nsolve = {"plain": a.nf, "analytic": a.nf, "analytic_gvd": a.nf, "fd3": 3 * a.nf}
+    nsolve = {"plain": a.nf, "analytic": a.nf, "analytic_gvd": a.nf, "gvd_eps": a.nf, "group_eps": a.nf, "fd3": 3 * a.nf}
     N, M = a.n * a.n, wl.mode_spec.num_modes
     # one derivative pass reads, per (problem, mode), the real fp64 Ritz vector (2N x 8 B) and the three coefficient fields
     # (exx, eyy, 1/ezz: 3N x 8 B; shared by the sweep, counted once per mode pass as they are re-read)
     bytes_pass = a.nf * M * (2 * N * 8 + 3 * N * 8)
     extra_ms = (np.median(dev["analytic"]) - np.median(dev["plain"]))
     gvd_ms = (np.median(dev["analytic_gvd"]) - np.median(dev["analytic"]))
+    gmap_ms = (np.median(dev["group_eps"]) - np.median(dev["gvd_eps"]))
     # the eigen-solves of the two arms are bit-identical, so the difference of the summed inner iterations is the correction
     # solves' (per problem: the slowest problem of its device batch, as for the eigen-solve's own counters)
     corr_iters = (np.median(inner["analytic_gvd"]) - np.median(inner["analytic"])) / (a.nf * M)
@@ -101,6 +108,7 @@ def main():
         device_ms_median={k: float(np.median(v)) for k, v in dev.items()},
         derivative_pass_device_ms_per_problem=float(extra_ms / a.nf),
         dispersion_pass_device_ms_per_problem=float(gvd_ms / a.nf),
+        group_gradient_map_device_ms_per_problem=float(gmap_ms / a.nf), group_gradient_map_finite=bool(gmap_finite),
         correction_inner_iters_per_mode=float(corr_iters),
         correction_residual_max=float(res_gvd.max()),
         derivative_pass_bytes=bytes_pass,
