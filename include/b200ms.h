@@ -29,7 +29,7 @@
 extern "C" {
 #endif
 
-#define B200MS_VERSION 207
+#define B200MS_VERSION 208
 
 /* return codes */
 enum {
@@ -163,7 +163,9 @@ typedef struct {
   double *overlap_prev;  /* NULL, or caller-allocated num_modes^2 complex128 (re,im), row-major [m_prev][m]: modal overlap
                             dot(mode m_prev of the PREVIOUS problem of this call, mode m of this one) (monitor_data.py:640-697,
                             after gauge/normalisation), the input of overlap_sort (monitor_data.py:1295-1375).  Zeros when
-                            there is no previous problem or its shape / num_modes / precision differ */
+                            there is no previous problem or its shape / num_modes / precision differ.  Post-processing (post,
+                            flux, te_fraction, overlap_prev) covers up to 64 modes: a problem with more that asks for any of it
+                            gets status B200MS_ERR_ARG ("post-processing supports at most 64 modes") */
   int eps_spec;          /* out: B200MS_SPEC_* */
   int status;            /* out: per-problem B200MS_* code */
   int converged;         /* out: number of converged modes */
@@ -372,6 +374,30 @@ int b200ms_debug_apply(b200ms_handle *h, const b200ms_problem *prob, int level, 
 int b200ms_debug_vcycle(b200ms_handle *h, const b200ms_problem *prob, const double *r, double *z);
 int b200ms_debug_solve(b200ms_handle *h, const b200ms_problem *prob, const double *b, double *x,
                        int *iters, double *relres);
+/* Since version 208.  One Krylov vector operation of the eigen-solver on caller data (GPU tests compare it with the model
+ * oracle/krylov_model.py), on a device batch built like b200ms_debug_batch's, through the solver's own member function and in the
+ * buffers it uses.  len = 2 nx ny (4 nx ny tensorial); a "vector set" is nprob consecutive complex128 (re,im) vectors of len, and
+ * V holds nv of them ([nv][nprob][len]).  prec 0: the Krylov element type (fp64 / complex128), 1: the multigrid precision (fp32 /
+ * complex64 with mg_precision 1; not for tensorial problems); inputs are rounded to that type.
+ *   what 0: inner CGS2 Gram-Schmidt (gs_dots, gs_update_dots / gs_update_norm, gs_scale) of w against V, 1 <= nv <= restart.
+ *           out: 2 vector sets, w'' / ||w''|| and its copy into the multigrid input (prec 1 with mg_precision 1; else zeros);
+ *           coef: [nprob][nv + 1] complex, the exported h_i (both passes summed), then ||w''||^2.
+ *   what 1 / 5 / 6: outer orthonormalisation of w against V (1 <= nv <= m; what 1 nv + 2 <= 64): 1 the device version with the
+ *           DGKS test, 5 the round-1 classical Gram-Schmidt with two passes, 6 with a second pass on cancellation only.  prec 0.
+ *           iused: [nprob + 1], in: nonzero = problem skipped by the second-pass test; out iused[nprob]: 1 if the second pass
+ *           ran (what 1; -1 otherwise).  out: 1 vector set, the normalised vector; coef: [nprob][nv + 1] complex, h, then ||w'||.
+ *   what 2: least-squares problem of one FGMRES cycle (fgmres_lsq_kernel) over kc = nv <= restart columns.  coef (in):
+ *           [nprob][kc][kc + 1] complex Hessenberg columns, column j = h_0j..h_jj, then ||w_j||^2 (real part read); res (in):
+ *           tolerance per problem (< 0: inactive), (out): the residual estimate; out: y [nprob][kc] complex; iused: columns used.
+ *   what 3: iterative-refinement step: w = r (fp64), V = Z (1 <= nv <= restart, in the prec type), coef (in) = y [nprob][nv]
+ *           complex; iused (in, may be NULL): nonzero = problem skipped.  out: 2 vector sets, r / ||r|| (ir_begin_kernel, 0 when
+ *           skipped) and r + ||r|| sum_k y_k Z_k (ir_update_kernel applied to x = r); res (out): ||r||^2.
+ *   what 4: lincomb (restart / Ritz-vector combination): out_q = sum_i Q[b][i][q] V_i for q < nk, V with 1 <= nv <= m + 1,
+ *           coef (in) = Q [nprob][nv][qld] complex, iused (in) = {nk, qld}, nk <= qld, nk <= max(restart, m).  prec 0.
+ *           out: nk vector sets.
+ * restart and m are the batch's: gmres_restart (clamped to 60) and the Krylov-Schur basis size (ncv, default max(2k+1, 20)). */
+int b200ms_debug_krylov(b200ms_handle *h, int nprob, const b200ms_problem *probs, int what, int prec, int nv, const double *V,
+                        const double *w, double *out, double *coef, int *iused, double *res);
 
 #ifdef __cplusplus
 }

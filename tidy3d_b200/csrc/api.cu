@@ -582,7 +582,7 @@ void post_overlaps(b200ms_handle *h, const b200ms_problem *prob, b200ms_result *
     std::fill(res[i].overlap_prev, res[i].overlap_prev + (size_t)2 * M * M, 0.0);
     if (i == 0 || !dev_fields[i] || !dev_fields[i - 1]) continue;
     const b200ms_problem &a = prob[i - 1], &b = prob[i];
-    if (a.nx != b.nx || a.ny != b.ny || a.num_modes != b.num_modes || (a.precision == 1) != (b.precision == 1) || M > 32) continue;
+    if (a.nx != b.nx || a.ny != b.ny || a.num_modes != b.num_modes || (a.precision == 1) != (b.precision == 1)) continue;
     todo.push_back(i);
   }
   // one launch per (shape, precision) run of jobs; jobs are few and small, so they are simply processed one shape at a time
@@ -1289,6 +1289,10 @@ extern "C" int b200ms_solve_batch(b200ms_handle *h, int nprob, const b200ms_prob
                   : s.relative ? "mode derivatives: the relative mode solver (basis fields) is not supported"
                                : "mode derivatives: removed PEC unknowns (mu_cross / split_curl_scaling with PEC cells) are not supported";
           }
+          if (res[i].status == B200MS_OK && (prob[i].post || res[i].flux || res[i].te_fraction || res[i].overlap_prev) && s.num_modes > kPostMaxModes) {
+            res[i].status = B200MS_ERR_ARG;
+            err = "post-processing supports at most 64 modes";
+          }
           if (res[i].status != B200MS_OK) {
             if (first_err == B200MS_OK) {
               first_err = res[i].status;
@@ -1702,6 +1706,28 @@ int debug_run(b200ms_handle *h, const Window &W, int what, int level, int mode, 
   return B200MS_OK;
 }
 
+// the problems set up as one device batch, formed only where b200ms_solve_batch would form it: the same group key for every
+// problem (B200MS_OK, else the status with h->err set)
+int debug_window(b200ms_handle *h, int nprob, const b200ms_problem *prob, const char *hook, Window &W) {
+  prepare_window(h, prob, 0, nprob, h->raw[0], h->stream, W);
+  for (const ProblemSetup &s : W.setups)
+    if (s.status != B200MS_OK) {
+      h->err = s.error;
+      return s.status;
+    }
+  const GroupKey k0 = group_key(W.setups[0], prob[0]);
+  for (int q = 1; q < nprob; ++q) {
+    const GroupKey kq = group_key(W.setups[q], prob[q]);
+    if (k0 < kq || kq < k0) {
+      h->err = std::string(hook) + ": problem " + std::to_string(q) +
+               " differs from problem 0 in what b200ms_solve_batch groups by (shape, modes, arithmetic kind, mu, symmetry, bend axis, "
+               "direction, basis, tensorial kind, precision, PEC masking, angles)";
+      return B200MS_ERR_ARG;
+    }
+  }
+  return B200MS_OK;
+}
+
 int debug_dispatch(b200ms_handle *h, int nprob, const b200ms_problem *prob, int what, int level, int mode, const double *in0,
                    const double *in1, double *out, int *iters, double *relres) {
   if (!h || nprob < 1 || !prob || !in0 || !out || what < 0 || what > 2) return B200MS_ERR_ARG;
@@ -1709,24 +1735,8 @@ int debug_dispatch(b200ms_handle *h, int nprob, const b200ms_problem *prob, int 
   h->err.clear();
   try {
     Window W;
-    prepare_window(h, prob, 0, nprob, h->raw[0], h->stream, W);
-    for (const ProblemSetup &s : W.setups)
-      if (s.status != B200MS_OK) {
-        h->err = s.error;
-        return s.status;
-      }
-    // one device batch, formed only where b200ms_solve_batch would form it: the same group key for every problem
+    if (const int rc = debug_window(h, nprob, prob, "b200ms_debug_batch", W)) return rc;
     const ProblemSetup &s = W.setups[0];
-    const GroupKey k0 = group_key(s, prob[0]);
-    for (int q = 1; q < nprob; ++q) {
-      const GroupKey kq = group_key(W.setups[q], prob[q]);
-      if (k0 < kq || kq < k0) {
-        h->err = "b200ms_debug_batch: problem " + std::to_string(q) +
-                 " differs from problem 0 in what b200ms_solve_batch groups by (shape, modes, arithmetic kind, mu, symmetry, bend axis, "
-                 "direction, basis, tensorial kind, precision, PEC masking, angles)";
-        return B200MS_ERR_ARG;
-      }
-    }
     const bool f32 = h->opt.mg_precision == 1;
     switch (kind_of(s)) {
       case 0:
@@ -1744,7 +1754,50 @@ int debug_dispatch(b200ms_handle *h, int nprob, const b200ms_problem *prob, int 
     return B200MS_ERR_CUDA;
   }
 }
+
+template <typename T, typename C, typename P, typename PC>
+int krylov_run(b200ms_handle *h, const Window &W, int what, int prec, int nv, const double *V, const double *w, double *out, double *coef,
+               int *iused, double *res) {
+  const int B = W.i1 - W.i0;
+  std::vector<int> ids(B);
+  for (int b = 0; b < B; ++b) ids[b] = b;
+  std::vector<const ProblemSetup *> ps;
+  std::vector<MediumRef> refs;
+  const bool share = batch_refs(W, ids, ps, refs);
+  BatchSolver<T, C, P, PC> S(h->arena, h->stream, h->opt);
+  S.build(ps, share, upload_refs(h, refs, h->stream));
+  const int rc = prec ? S.template debug_krylov<P>(what, nv, V, w, out, coef, iused, res) : S.template debug_krylov<T>(what, nv, V, w, out, coef, iused, res);
+  if (rc != B200MS_OK) h->err = "b200ms_debug_krylov: arguments out of range for this batch (what " + std::to_string(what) + ", prec " + std::to_string(prec) +
+                                ", nv " + std::to_string(nv) + ", restart " + std::to_string(S.restart) + ", m " + std::to_string(S.m) + ")";
+  return rc;
+}
 }  // namespace
+
+extern "C" int b200ms_debug_krylov(b200ms_handle *h, int nprob, const b200ms_problem *probs, int what, int prec, int nv, const double *V,
+                                   const double *w, double *out, double *coef, int *iused, double *res) {
+  if (!h || nprob < 1 || !probs || prec < 0 || prec > 1) return B200MS_ERR_ARG;
+  if (cudaSetDevice(h->device) != cudaSuccess) return B200MS_ERR_CUDA;
+  h->err.clear();
+  try {
+    Window W;
+    if (const int rc = debug_window(h, nprob, probs, "b200ms_debug_krylov", W)) return rc;
+    const bool f32 = h->opt.mg_precision == 1;
+    switch (kind_of(W.setups[0])) {
+      case 0:
+        return f32 ? krylov_run<double, double, float, float>(h, W, what, prec, nv, V, w, out, coef, iused, res)
+                   : krylov_run<double, double, double, double>(h, W, what, prec, nv, V, w, out, coef, iused, res);
+      case 1:
+        return f32 ? krylov_run<cplx, double, cplxf, float>(h, W, what, prec, nv, V, w, out, coef, iused, res)
+                   : krylov_run<cplx, double, cplx, double>(h, W, what, prec, nv, V, w, out, coef, iused, res);
+      default:
+        return f32 ? krylov_run<cplx, cplx, cplxf, cplxf>(h, W, what, prec, nv, V, w, out, coef, iused, res)
+                   : krylov_run<cplx, cplx, cplx, cplx>(h, W, what, prec, nv, V, w, out, coef, iused, res);
+    }
+  } catch (const std::exception &e) {
+    h->err = e.what();
+    return B200MS_ERR_CUDA;
+  }
+}
 
 extern "C" int b200ms_debug_batch(b200ms_handle *h, int nprob, const b200ms_problem *probs, int what, int level, int mode,
                                   const double *in, const double *in2, double *out, int *iters, double *relres) {

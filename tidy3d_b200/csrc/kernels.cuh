@@ -1074,14 +1074,15 @@ __global__ void __launch_bounds__(256) multiaxpy_kernel(const T *V, size_t vstri
   }
 }
 
-// out_k[b] = sum_i Q[b][i][k] * V_i[b],  k in [0, nk); Q row-major [nv][qld]
+// out_k[b] = sum_i Q[b][i][k] * V_i[b],  k in [0, nk); Q row-major [nv][qld] per problem, of which the first nk columns
+// are staged in shared memory (nv * nk elements)
 template <typename T>
 __global__ void __launch_bounds__(256) lincomb_kernel(const T *V, size_t vstride, size_t len, const T *Q, int nv,
                                                       int nk, int qld, T *out, size_t ostride) {
   const int b = blockIdx.y;
   extern __shared__ unsigned char smem_raw[];
   T *sq = reinterpret_cast<T *>(smem_raw);
-  for (int i = threadIdx.x; i < nv * qld; i += 256) sq[i] = Q[(size_t)b * nv * qld + i];
+  for (int t = threadIdx.x; t < nv * nk; t += 256) sq[t] = Q[(size_t)b * nv * qld + (size_t)(t / nk) * qld + t % nk];
   __syncthreads();
   const size_t stride = (size_t)gridDim.x * 256;
   for (size_t e = (size_t)blockIdx.x * 256 + threadIdx.x; e < len; e += stride) {
@@ -1093,7 +1094,7 @@ __global__ void __launch_bounds__(256) lincomb_kernel(const T *V, size_t vstride
         const T v = ldg(V + (size_t)i * vstride + (size_t)b * len + e);
 #pragma unroll
         for (int k = 0; k < 8; ++k)
-          if (k0 + k < nk) acc[k] += sq[i * qld + k0 + k] * v;
+          if (k0 + k < nk) acc[k] += sq[i * nk + k0 + k] * v;
       }
 #pragma unroll
       for (int k = 0; k < 8; ++k)

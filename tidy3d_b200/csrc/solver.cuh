@@ -165,6 +165,16 @@ class BatchSolver {
     if (opt_.inner_mode != 0) restart = std::min(restart, kGsMaxCoef - 4);
     mask_x_ = (!p0.ax[0].pmc && nx > 1) ? 1 : 0;
     mask_y_ = (!p0.ax[1].pmc && ny > 1) ? 1 : 0;
+    {  // lincomb_kernel stages up to m x m coefficients per CTA: beyond the 48 KB default it has to opt in (see lincomb)
+      int dev = 0, optin = 0;
+      CUDA_CHECK(cudaGetDevice(&dev));
+      CUDA_CHECK(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
+      lincomb_smem_ = std::min<size_t>((size_t)optin, std::max<size_t>(48 * 1024, (size_t)m * m * sizeof(T)));
+      cudaFuncAttributes fa;
+      CUDA_CHECK(cudaFuncGetAttributes(&fa, lincomb_kernel<T>));
+      if (lincomb_smem_ > (size_t)fa.maxDynamicSharedSizeBytes)
+        CUDA_CHECK(cudaFuncSetAttribute(lincomb_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)lincomb_smem_));
+    }
 
     // hierarchy geometry from problem 0; indefinite shifts limit the coarsest spacing
     double kh_limit = 0.0, kmax = 0.0;
@@ -203,7 +213,7 @@ class BatchSolver {
     }
     sz.add<T>((size_t)(m + 1) * vstride);        // outer basis
     sz.add<T>((size_t)(restart + 1) * vstride);  // FGMRES V
-    sz.add<T>((size_t)restart * vstride);        // FGMRES Z
+    sz.add<T>((size_t)scratch_slots() * vstride);  // FGMRES Z, and the scratch of the Krylov-Schur restart and the Ritz vectors
     sz.add<T>(vstride * 4);                      // xsol, rhs scratch, preconditioner scratch
     sz.add<T>((size_t)k * vstride);              // Ritz vectors
     sz.add<T>((size_t)B * kDotChunks * pstride());
@@ -351,7 +361,7 @@ class BatchSolver {
     // Krylov storage
     Vout_ = arena_.get<T>((size_t)(m + 1) * vstride);
     Vg_ = arena_.get<T>((size_t)(restart + 1) * vstride);
-    Zg_ = arena_.get<T>((size_t)restart * vstride);
+    Zg_ = arena_.get<T>((size_t)scratch_slots() * vstride);
     xsol_ = arena_.get<T>(vstride);
     rhs_ = arena_.get<T>(vstride);
     pre_a_ = arena_.get<P>(vstride);
@@ -1135,6 +1145,8 @@ class BatchSolver {
   int pstride() const { return std::max(m, restart) + 2; }
   int hstride() const { return 2 * (std::max(m, restart) + 2) + 2; }
   int vec_blocks() const { return (int)std::min<size_t>((len + 255) / 256, 1024); }
+  // vector slots of Zg_: the FGMRES Z basis (restart), and the outputs of the restart (keep <= m - 1) and of the Ritz vectors (k <= m)
+  int scratch_slots() const { return std::max(restart, m); }
 
   // dst[b][off + i] (+)= <V_i, w>, i < nv   (vectors of length ln, basis stride vs)
   template <typename U>
@@ -1161,6 +1173,20 @@ class BatchSolver {
     stats.launches++;
     dim3 grd((unsigned)std::min<size_t>((ln + 255) / 256, 1024), B);
     scale_kernel<U><<<grd, 256, 0, st_>>>(x, y, ln, nrm2, stride, 1);
+  }
+  // out_q[b] = sum_i Q[b][i][q] V_i[b] for q < nk (Q: [B][nv][qld], V with slot stride vs, out with slot stride os).  The
+  // columns of Q go in tiles whose nv x tile coefficients fit in a CTA's shared memory; every output sums over i in the same
+  // order whatever the tiling.
+  void lincomb(const T *V, size_t vs, const T *Q, int nv, int nk, int qld, T *out, size_t os) {
+    const int tile = (int)std::min<size_t>(nk, lincomb_smem_ / ((size_t)nv * sizeof(T)));
+    if (tile < 1) throw std::runtime_error("lincomb: the coefficients of " + std::to_string(nv) + " basis vectors exceed shared memory");
+    dim3 grd(vec_blocks(), B);
+    for (int k0 = 0; k0 < nk; k0 += tile) {
+      const int nt = std::min(tile, nk - k0);
+      lincomb_kernel<T><<<grd, 256, (size_t)nv * nt * sizeof(T), st_>>>(V, vs, len, Q + k0, nv, nt, qld, out + (size_t)k0 * os, os);
+      stats.launches++;
+      CUDA_CHECK(cudaGetLastError());
+    }
   }
   void copy(const T *src, T *dst) { CUDA_CHECK(cudaMemcpyAsync(dst, src, vstride * sizeof(T), cudaMemcpyDeviceToDevice, st_)); }
   void fetch_h(size_t count) {
@@ -1406,6 +1432,34 @@ class BatchSolver {
     }
     k_scale<U>(w, dst, dst2, ln, P2, nch, hexp, hstride, nv);
   }
+  // least-squares problem of an FGMRES cycle over the first kc columns of Hd_ (type U, tolerances in tol_dev_) -> y in ydev_,
+  // estimates in res_dev_, columns used in jused_dev_
+  template <typename U>
+  void k_lsq(int kc) {
+    fgmres_lsq_kernel<U><<<(B + 31) / 32, 32, 0, st_>>>(reinterpret_cast<const U *>(Hd_), restart, restart + 4, kc, tol_dev_, lsq_work_,
+                                                        reinterpret_cast<U *>(ydev_), restart, res_dev_, jused_dev_, B);
+    stats.launches++;
+  }
+  // refinement step, begin: Vg_ slot 0 (type U) = r / ||r|| (0 for the problems flagged in skip_dev_), also into the multigrid
+  // input lv[0].b when U is the multigrid precision of a mixed solver; ||r||^2 (partials in gpart<T>(0)) -> n2out
+  template <typename U>
+  void k_ir_begin(const T *r, int nch, double *n2out) {
+    const dim3 egrd((unsigned)stream_blocks(len), B);
+    U *Vu = reinterpret_cast<U *>(Vg_), *rp2 = nullptr;
+    if constexpr (kMixed && std::is_same<U, P>::value) rp2 = lv[0].b;
+    stats.launches++;
+    if (vec_ok<U>(len)) ir_begin_kernel<T, U, PackTraits<U>::EPV><<<egrd, 256, 0, st_>>>(r, Vu, rp2, len, gpart<T>(0), nch, pstride(), 0, n2out, skip_dev_);
+    else ir_begin_kernel<T, U, 1><<<egrd, 256, 0, st_>>>(r, Vu, rp2, len, gpart<T>(0), nch, pstride(), 0, n2out, skip_dev_);
+  }
+  // refinement step, end: x += sqrt(n2) sum_{k<nv} y_k Z_k with Z in Zg_ and y in ydev_ (type U)
+  template <typename U>
+  void k_ir_update(int nv, const double *n2, T *x) {
+    const dim3 egrd((unsigned)stream_blocks(len), B);
+    const U *Zu = reinterpret_cast<const U *>(Zg_), *yu = reinterpret_cast<const U *>(ydev_);
+    stats.launches++;
+    if (vec_ok<U>(len)) ir_update_kernel<T, U, PackTraits<U>::EPV><<<egrd, 256, 0, st_>>>(Zu, vstride, len, yu, restart, nv, n2, x);
+    else ir_update_kernel<T, U, 1><<<egrd, 256, 0, st_>>>(Zu, vstride, len, yu, restart, nv, n2, x);
+  }
   // outer (Krylov-Schur) orthonormalisation through the device kernels.  Classical Gram-Schmidt with the DGKS test
   // ARPACK uses (dgetv0/dnaitr: reorthogonalise when ||w'|| < 0.717 ||w||): the second pass -- two more reads of the
   // whole fp64 basis -- runs only when some active problem needs it.
@@ -1487,7 +1541,6 @@ class BatchSolver {
   template <typename U>
   int fgmres_cycle(const std::vector<double> &tol, std::vector<double> &res, std::vector<int> &jused, bool staged, int budget) {
     U *Vu = reinterpret_cast<U *>(Vg_), *Zu = reinterpret_cast<U *>(Zg_), *Hu = reinterpret_cast<U *>(Hd_);
-    U *yu = reinterpret_cast<U *>(ydev_);
     const int ld = restart + 4;
     constexpr bool kStage = kMixed && std::is_same<U, P>::value;
     CUDA_CHECK(cudaMemcpyAsync(tol_dev_, tol.data(), B * sizeof(double), cudaMemcpyHostToDevice, st_));
@@ -1509,8 +1562,7 @@ class BatchSolver {
         apply_true_u<U>(MODE_APPLY, zj, nullptr, w);
         gs_cgs2<U>(Vu, vstride, len, j + 1, w, w, kStage ? reinterpret_cast<U *>(lv[0].b) : nullptr, Hu + (size_t)j * ld, (size_t)restart * ld);
       }
-      fgmres_lsq_kernel<U><<<(B + 31) / 32, 32, 0, st_>>>(Hu, restart, ld, j, tol_dev_, lsq_work_, yu, restart, res_dev_, jused_dev_, B);
-      stats.launches++;
+      k_lsq<U>(j);
       CUDA_CHECK(cudaMemcpyAsync(hres.data(), res_dev_, B * sizeof(double), cudaMemcpyDeviceToHost, st_));
       CUDA_CHECK(cudaMemcpyAsync(hju.data(), jused_dev_, B * sizeof(int), cudaMemcpyDeviceToHost, st_));
       CUDA_CHECK(cudaStreamSynchronize(st_));
@@ -1558,7 +1610,6 @@ class BatchSolver {
     const int nch = gs_chunks(len);
     int total = 0, cyc = 0;
     bool verified = true;
-    const dim3 egrd((unsigned)stream_blocks(len), B);
     while (true) {
       // ||r||^2 of the current residual (partials; reduced inside ir_begin)
       k_dots<T>(rcur, vstride, len, rcur, 1, gpart<T>(0), 0, nch);
@@ -1586,35 +1637,20 @@ class BatchSolver {
         tolc[b] = done[b] ? -1.0 : std::min(0.5, std::max(want, ir ? opt_.ir_floor : 0.0));
       }
       CUDA_CHECK(cudaMemcpyAsync(skip_dev_, hskip.data(), B, cudaMemcpyHostToDevice, st_));
-      stats.launches++;
       double *n2cur = cyc == 0 ? bn2_dev_ : n2_dev_;  // ||r||^2 of this cycle (cycle 0: ||b||^2, kept for the relative residuals)
       int steps;
       if (ir) {
-        P *Vp = reinterpret_cast<P *>(Vg_);
-#define B200_IRB(E) ir_begin_kernel<T, P, E><<<egrd, 256, 0, st_>>>(rcur, Vp, lv[0].b, len, gpart<T>(0), nch, pstride(), 0, n2cur, skip_dev_)
-        if (vec_ok<P>(len)) B200_IRB(PackTraits<P>::EPV); else B200_IRB(1);
-#undef B200_IRB
+        k_ir_begin<P>(rcur, nch, n2cur);
         steps = fgmres_cycle<P>(tolc, cres, ju, true, opt_.gmres_maxit - total);
         int nvmax = 0;
         for (int b = 0; b < B; ++b) nvmax = std::max(nvmax, ju[b]);
-        if (nvmax > 0) {
-          stats.launches++;
-          const P *Zp = reinterpret_cast<const P *>(Zg_), *yp = reinterpret_cast<const P *>(ydev_);
-          if (vec_ok<P>(len)) ir_update_kernel<T, P, PackTraits<P>::EPV><<<egrd, 256, 0, st_>>>(Zp, vstride, len, yp, restart, nvmax, n2cur, xsol);
-          else ir_update_kernel<T, P, 1><<<egrd, 256, 0, st_>>>(Zp, vstride, len, yp, restart, nvmax, n2cur, xsol);
-        }
+        if (nvmax > 0) k_ir_update<P>(nvmax, n2cur, xsol);
       } else {
-#define B200_IRB(E) ir_begin_kernel<T, T, E><<<egrd, 256, 0, st_>>>(rcur, Vg_, nullptr, len, gpart<T>(0), nch, pstride(), 0, n2cur, skip_dev_)
-        if (vec_ok<T>(len)) B200_IRB(PackTraits<T>::EPV); else B200_IRB(1);
-#undef B200_IRB
+        k_ir_begin<T>(rcur, nch, n2cur);
         steps = fgmres_cycle<T>(tolc, cres, ju, false, opt_.gmres_maxit - total);
         int nvmax = 0;
         for (int b = 0; b < B; ++b) nvmax = std::max(nvmax, ju[b]);
-        if (nvmax > 0) {
-          stats.launches++;
-          if (vec_ok<T>(len)) ir_update_kernel<T, T, PackTraits<T>::EPV><<<egrd, 256, 0, st_>>>(Zg_, vstride, len, ydev_, restart, nvmax, n2cur, xsol);
-          else ir_update_kernel<T, T, 1><<<egrd, 256, 0, st_>>>(Zg_, vstride, len, ydev_, restart, nvmax, n2cur, xsol);
-        }
+        if (nvmax > 0) k_ir_update<T>(nvmax, n2cur, xsol);
       }
       total += steps;
       // estimates: res_cycle is relative to the residual the cycle started from
@@ -1693,14 +1729,8 @@ class BatchSolver {
   void init_start_from(const T *warm, int Bw) {
     std::vector<T> ones((size_t)B * k, from_real<T>(1.0));
     CUDA_CHECK(cudaMemcpyAsync(qbuf_, ones.data(), ones.size() * sizeof(T), cudaMemcpyHostToDevice, st_));
-    if (Bw == B) {
-      dim3 grd(vec_blocks(), B);
-      lincomb_kernel<T><<<grd, 256, (size_t)k * sizeof(T), st_>>>(warm, vstride, len, qbuf_, k, 1, 1, rhs_, vstride);
-    } else {  // a shorter last window: problem b starts from problem b of the previous window (Bw >= B)
-      dim3 grd(vec_blocks(), B);
-      lincomb_kernel<T><<<grd, 256, (size_t)k * sizeof(T), st_>>>(warm, (size_t)Bw * len, len, qbuf_, k, 1, 1, rhs_, vstride);
-    }
-    stats.launches++;
+    // a shorter last window (Bw > B): problem b starts from problem b of the previous window
+    lincomb(warm, (size_t)Bw * len, qbuf_, k, 1, 1, rhs_, vstride);
     if (!tensor_) mask_E(rhs_, len);
     dots(rhs_, 1, rhs_, hbuf_, hstride(), 0, false);
     scale_inv_norm(rhs_, Vout_, hbuf_, hstride());
@@ -1872,10 +1902,7 @@ class BatchSolver {
       // V[:, :keep] <- V Q ; V[keep] <- V[m]      (Zg_ is free between inner solves: scratch)
       const int keep = keep_of(keep_target);
       CUDA_CHECK(cudaMemcpyAsync(qbuf_, qh.data(), qh.size() * sizeof(T), cudaMemcpyHostToDevice, st_));
-      {
-        dim3 grd(vec_blocks(), B);
-        lincomb_kernel<T><<<grd, 256, (size_t)m * m * sizeof(T), st_>>>(Vout_, vstride, len, qbuf_, m, keep, m, Zg_, vstride);
-      }
+      lincomb(Vout_, vstride, qbuf_, m, keep, m, Zg_, vstride);
       CUDA_CHECK(cudaMemcpyAsync(Vout_, Zg_, (size_t)keep * vstride * sizeof(T), cudaMemcpyDeviceToDevice, st_));
       CUDA_CHECK(cudaMemcpyAsync(Vout_ + (size_t)keep * vstride, Vout_ + (size_t)m * vstride, vstride * sizeof(T),
                                  cudaMemcpyDeviceToDevice, st_));
@@ -1913,10 +1940,7 @@ class BatchSolver {
         }
       }
     CUDA_CHECK(cudaMemcpyAsync(qbuf_, yh.data(), yh.size() * sizeof(T), cudaMemcpyHostToDevice, st_));
-    {
-      dim3 grd(vec_blocks(), B);
-      lincomb_kernel<T><<<grd, 256, (size_t)m * k * sizeof(T), st_>>>(Vout_, vstride, len, qbuf_, m, k, k, Zg_, vstride);
-    }
+    lincomb(Vout_, vstride, qbuf_, m, k, k, Zg_, vstride);
     for (int b : which)
       for (int q = 0; q < k; ++q)
         CUDA_CHECK(cudaMemcpyAsync(ritz_ + (size_t)q * vstride + (size_t)b * len, Zg_ + (size_t)q * vstride + (size_t)b * len,
@@ -1969,10 +1993,7 @@ class BatchSolver {
       }
     }
     CUDA_CHECK(cudaMemcpyAsync(qbuf_, yh.data(), yh.size() * sizeof(T), cudaMemcpyHostToDevice, st_));
-    {
-      dim3 grd(vec_blocks(), B);
-      lincomb_kernel<T><<<grd, 256, (size_t)k * k * sizeof(T), st_>>>(Vout_, vstride, len, qbuf_, k, k, k, ritz_, vstride);
-    }
+    lincomb(Vout_, vstride, qbuf_, k, k, k, ritz_, vstride);
     CUDA_CHECK(cudaStreamSynchronize(st_));
     return vals;
   }
@@ -2005,10 +2026,7 @@ class BatchSolver {
     for (int b = 0; b < B; ++b)
       for (int q = 0; q < k; ++q) ph[((size_t)b * k + perm[(size_t)b * k + q]) * k + q] = from_real<T>(1.0);
     CUDA_CHECK(cudaMemcpyAsync(qbuf_, ph.data(), ph.size() * sizeof(T), cudaMemcpyHostToDevice, st_));
-    {
-      dim3 grd(vec_blocks(), B);
-      lincomb_kernel<T><<<grd, 256, (size_t)k * k * sizeof(T), st_>>>(ritz_, vstride, len, qbuf_, k, k, k, Zg_, vstride);
-    }
+    lincomb(ritz_, vstride, qbuf_, k, k, k, Zg_, vstride);
     if (!want_fields) {
       CUDA_CHECK(cudaStreamSynchronize(st_));
       return;
@@ -2063,6 +2081,147 @@ class BatchSolver {
   size_t output_bytes_per_problem() const { return (size_t)6 * N * k * (single_out_ ? sizeof(cplxf) : sizeof(cplx)); }
   T *hessenberg() { return Hd_; }
   T *ritz_ptr() { return ritz_; }
+
+  // ---- b200ms_debug_krylov: one Krylov vector operation of this batch on caller data, through the member function the
+  // solver runs, in the buffers it runs it in (include/b200ms.h documents what / nv / the arrays).  U: T, or P for the
+  // inner-solver operations in the multigrid precision.  Host vectors are complex (re,im); slot i of problem b at (i B + b) len.
+  template <typename U>
+  int debug_krylov(int what, int nv, const double *V, const double *w, double *out, double *coef, int *iused, double *res) {
+    auto put = [&](const double *src, size_t n, U *dst) {
+      std::vector<U> a(n);
+      for (size_t e = 0; e < n; ++e) a[e] = from_cd<U>(cd(src[2 * e], src[2 * e + 1]));
+      CUDA_CHECK(cudaMemcpy(dst, a.data(), n * sizeof(U), cudaMemcpyHostToDevice));
+    };
+    auto get = [&](const U *src, size_t n, double *dst) {
+      std::vector<U> a(n);
+      CUDA_CHECK(cudaMemcpy(a.data(), src, n * sizeof(U), cudaMemcpyDeviceToHost));
+      for (size_t e = 0; e < n; ++e) {
+        const cd v = to_cd(a[e]);
+        dst[2 * e] = v.real();
+        dst[2 * e + 1] = v.imag();
+      }
+    };
+    auto put_skip = [&]() {
+      std::vector<unsigned char> s(B, 0);
+      std::vector<char> sc(B, 0);
+      for (int b = 0; b < B && iused; ++b) s[b] = sc[b] = iused[b] != 0;
+      CUDA_CHECK(cudaMemcpy(skip_dev_, s.data(), B, cudaMemcpyHostToDevice));
+      return sc;
+    };
+    const size_t n1 = (size_t)B * len;
+    if (tensor_ && !std::is_same<U, T>::value) return B200MS_ERR_ARG;  // the tensorial solve runs no multigrid-precision Krylov cycles
+    if (what == 0) {  // inner CGS2 against slots 0..nv-1 of the FGMRES basis, w in slot nv, column nv-1 of the Hessenberg export
+      if (nv < 1 || nv > restart || !V || !w || !out || !coef) return B200MS_ERR_ARG;
+      U *Vu = reinterpret_cast<U *>(Vg_), *Hu = reinterpret_cast<U *>(Hd_), *wv = Vu + (size_t)nv * vstride;
+      U *dst2 = nullptr;  // fgmres_cycle: the multigrid input copy exists only for multigrid-precision cycles of a mixed solver
+      if constexpr (kMixed && std::is_same<U, P>::value) dst2 = lv[0].b;
+      for (int i = 0; i < nv; ++i) put(V + 2 * i * n1, n1, Vu + (size_t)i * vstride);
+      put(w, n1, wv);
+      const int ld = restart + 4;
+      CUDA_CHECK(cudaMemset(Hd_, 0, (size_t)B * restart * ld * sizeof(T)));
+      if (dst2) CUDA_CHECK(cudaMemset(dst2, 0, n1 * sizeof(U)));
+      gs_cgs2<U>(Vu, vstride, len, nv, wv, wv, dst2, Hu + (size_t)(nv - 1) * ld, (size_t)restart * ld);
+      CUDA_CHECK(cudaStreamSynchronize(st_));
+      CUDA_CHECK(cudaGetLastError());
+      get(wv, n1, out);
+      if (dst2) get(dst2, n1, out + 2 * n1);
+      else std::fill(out + 2 * n1, out + 4 * n1, 0.0);
+      for (int b = 0; b < B; ++b) get(Hu + ((size_t)b * restart + nv - 1) * ld, nv + 1, coef + 2 * (size_t)b * (nv + 1));
+      return B200MS_OK;
+    }
+    if (what == 1 || what == 5 || what == 6) {  // outer orthonormalisation against slots 0..nv-1 of the eigen-basis, w in slot nv
+      if constexpr (!std::is_same<U, T>::value) return B200MS_ERR_ARG;
+      else {
+        if (nv < 1 || nv > m || (what == 1 && nv + 2 > kGsMaxCoef) || !V || !w || !out || !coef || !iused) return B200MS_ERR_ARG;
+        for (int i = 0; i < nv; ++i) put(V + 2 * i * n1, n1, Vout_ + (size_t)i * vstride);
+        T *wv = Vout_ + (size_t)nv * vstride;
+        put(w, n1, wv);
+        const std::vector<char> skip = put_skip();
+        std::vector<cd> h;
+        std::vector<double> nrm;
+        const int before = stats.outer_second_pass;
+        if (what == 1) orthonormalise_dev(Vout_, nv, wv, wv, h, nrm, &skip);
+        else orthonormalise(Vout_, nv, wv, wv, h, nrm, what == 6, &skip);
+        CUDA_CHECK(cudaStreamSynchronize(st_));
+        CUDA_CHECK(cudaGetLastError());
+        get(wv, n1, out);
+        for (int b = 0; b < B; ++b) {
+          for (int i = 0; i <= nv; ++i) {
+            const cd v = i < nv ? h[(size_t)b * nv + i] : cd(nrm[b], 0.0);
+            coef[2 * ((size_t)b * (nv + 1) + i)] = v.real();
+            coef[2 * ((size_t)b * (nv + 1) + i) + 1] = v.imag();
+          }
+        }
+        iused[B] = what == 1 ? stats.outer_second_pass - before : -1;  // orthonormalise does not report it
+        return B200MS_OK;
+      }
+    }
+    if (what == 2) {  // least squares of a cycle over nv columns of a caller Hessenberg matrix [B][nv][nv + 1]
+      if (nv < 1 || nv > restart || !coef || !out || !iused || !res) return B200MS_ERR_ARG;
+      const int ld = restart + 4;
+      std::vector<double> hh((size_t)2 * B * restart * ld, 0.0);
+      for (int b = 0; b < B; ++b)
+        for (int j = 0; j < nv; ++j)
+          for (int i = 0; i <= j + 1; ++i) {
+            const size_t s = ((size_t)b * nv + j) * (nv + 1) + i, d = ((size_t)b * restart + j) * ld + i;
+            hh[2 * d] = coef[2 * s];
+            hh[2 * d + 1] = coef[2 * s + 1];
+          }
+      put(hh.data(), (size_t)B * restart * ld, reinterpret_cast<U *>(Hd_));
+      CUDA_CHECK(cudaMemcpy(tol_dev_, res, B * sizeof(double), cudaMemcpyHostToDevice));
+      k_lsq<U>(nv);
+      CUDA_CHECK(cudaStreamSynchronize(st_));
+      CUDA_CHECK(cudaGetLastError());
+      for (int b = 0; b < B; ++b) get(reinterpret_cast<const U *>(ydev_) + (size_t)b * restart, nv, out + 2 * (size_t)b * nv);
+      CUDA_CHECK(cudaMemcpy(res, res_dev_, B * sizeof(double), cudaMemcpyDeviceToHost));
+      CUDA_CHECK(cudaMemcpy(iused, jused_dev_, B * sizeof(int), cudaMemcpyDeviceToHost));
+      return B200MS_OK;
+    }
+    if (what == 3) {  // refinement step: r / ||r|| into the basis, then x = r + ||r|| sum_k y_k Z_k
+      if (nv < 1 || nv > restart || !V || !w || !coef || !out || !res) return B200MS_ERR_ARG;
+      std::vector<T> r(n1);
+      for (size_t e = 0; e < n1; ++e) r[e] = from_cd<T>(cd(w[2 * e], w[2 * e + 1]));
+      CUDA_CHECK(cudaMemcpy(rhs_, r.data(), n1 * sizeof(T), cudaMemcpyHostToDevice));
+      CUDA_CHECK(cudaMemcpy(xsol_, r.data(), n1 * sizeof(T), cudaMemcpyHostToDevice));
+      U *Zu = reinterpret_cast<U *>(Zg_);
+      for (int i = 0; i < nv; ++i) put(V + 2 * i * n1, n1, Zu + (size_t)i * vstride);
+      std::vector<double> y((size_t)2 * B * restart, 0.0);
+      for (int b = 0; b < B; ++b) std::copy(coef + 2 * (size_t)b * nv, coef + 2 * (size_t)(b + 1) * nv, y.begin() + 2 * (size_t)b * restart);
+      put(y.data(), (size_t)B * restart, reinterpret_cast<U *>(ydev_));
+      put_skip();
+      const int nch = gs_chunks(len);
+      k_dots<T>(rhs_, vstride, len, rhs_, 1, gpart<T>(0), 0, nch);
+      k_ir_begin<U>(rhs_, nch, n2_dev_);
+      k_ir_update<U>(nv, n2_dev_, xsol_);
+      CUDA_CHECK(cudaStreamSynchronize(st_));
+      CUDA_CHECK(cudaGetLastError());
+      get(reinterpret_cast<const U *>(Vg_), n1, out);
+      std::vector<T> x(n1);
+      CUDA_CHECK(cudaMemcpy(x.data(), xsol_, n1 * sizeof(T), cudaMemcpyDeviceToHost));
+      for (size_t e = 0; e < n1; ++e) {
+        out[2 * (n1 + e)] = to_cd(x[e]).real();
+        out[2 * (n1 + e) + 1] = to_cd(x[e]).imag();
+      }
+      CUDA_CHECK(cudaMemcpy(res, n2_dev_, B * sizeof(double), cudaMemcpyDeviceToHost));
+      return B200MS_OK;
+    }
+    if (what == 4) {  // out_q = sum_i Q[b][i][q] V_i, q < nk = iused[0], Q: [B][nv][qld = iused[1]]
+      if constexpr (!std::is_same<U, T>::value) return B200MS_ERR_ARG;
+      else {
+        if (!iused || !V || !coef || !out) return B200MS_ERR_ARG;
+        const int nk = iused[0], qld = iused[1];
+        if (nv < 1 || nv > m + 1 || nk < 1 || nk > qld || nk > scratch_slots() || (size_t)nv * qld > (size_t)(m + 1) * (m + 1)) return B200MS_ERR_ARG;
+        for (int i = 0; i < nv; ++i) put(V + 2 * i * n1, n1, Vout_ + (size_t)i * vstride);
+        put(coef, (size_t)B * nv * qld, qbuf_);
+        lincomb(Vout_, vstride, qbuf_, nv, nk, qld, Zg_, vstride);
+        CUDA_CHECK(cudaStreamSynchronize(st_));
+        CUDA_CHECK(cudaGetLastError());
+        get(Zg_, (size_t)nk * n1, out);
+        return B200MS_OK;
+      }
+    }
+    return B200MS_ERR_ARG;
+  }
 
  private:
   static void transfer_sizes(const AxisTransfer &t, size_t &ints, size_t &dbls) {
@@ -2163,6 +2322,7 @@ class BatchSolver {
   std::vector<cd> sig_mg_host_;
   bool dinv_ready_ = false;
   int sms_ = 0;  // streaming multiprocessors of the device
+  size_t lincomb_smem_ = 48 * 1024;  // dynamic shared memory lincomb_kernel may use (opted in by build)
   std::map<long, int> m2_resident_;  // pair-marching kernel: resident CTAs on the device per (mode, prefetch depth, CTA width)
   cudaGraphExec_t graph_exec_ = nullptr;
   P *graph_result_ = nullptr;
