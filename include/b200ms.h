@@ -29,7 +29,7 @@
 extern "C" {
 #endif
 
-#define B200MS_VERSION 208
+#define B200MS_VERSION 209
 
 /* return codes */
 enum {
@@ -398,6 +398,19 @@ int b200ms_debug_solve(b200ms_handle *h, const b200ms_problem *prob, const doubl
  * restart and m are the batch's: gmres_restart (clamped to 60) and the Krylov-Schur basis size (ncv, default max(2k+1, 20)). */
 int b200ms_debug_krylov(b200ms_handle *h, int nprob, const b200ms_problem *probs, int what, int prec, int nv, const double *V,
                         const double *w, double *out, double *coef, int *iused, double *res);
+/* Since version 209.  The field recovery of the eigen-solver (the epilogue: per-problem mode permutation, E / H recovery,
+ * direction sign, tensorial conjugate flip, angled / bend back-transform) on caller vectors, on a device batch built like
+ * b200ms_debug_batch's (GPU tests compare it with the model oracle/field_model.py).  k = num_modes, len = 2 nx ny (4 nx ny
+ * tensorial: Ex, Ey, Hx, Hy of the first-order operator).
+ *   vecs:     [k][nprob][len] complex128 (re,im), written into the Ritz vector slots (rounded to the solver's element type:
+ *             real-arithmetic problems drop the imaginary part).
+ *   ncomplex: [nprob][k] complex128, n_eff + i k_eff of output mode q in solver units (the delivered n_complex / knorm); the
+ *             tensorial recovery does not use it.
+ *   perm:     [nprob][k]: output mode q of problem b is Ritz slot perm[b][q] (a permutation of 0..k-1 per problem).
+ *   out:      nprob consecutive blocks of 6 nx ny k elements in the layout of b200ms_result.fields ([2][3][nx][ny][k]),
+ *             complex128, or complex64 when the problems have precision 1. */
+int b200ms_debug_fields(b200ms_handle *h, int nprob, const b200ms_problem *probs, const double *vecs, const double *ncomplex,
+                        const int *perm, void *out);
 
 #ifdef __cplusplus
 }

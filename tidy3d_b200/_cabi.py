@@ -17,7 +17,7 @@ import numpy as np
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("B200MS_LIB") or os.path.join(_HERE, "libb200ms.so")  # B200MS_LIB: developer override (A/B of builds)
 
-ABI_VERSION = 208  # B200MS_VERSION of include/b200ms.h
+ABI_VERSION = 209  # B200MS_VERSION of include/b200ms.h
 OK, ERR_SHAPE, ERR_NO_MODES, ERR_UNSUPPORTED, ERR_CUDA, ERR_NOCONV, ERR_ARG = range(7)
 SPEC_NAMES = {0: "diagonal", 1: "tensorial_real", 2: "tensorial_complex"}
 
@@ -72,7 +72,7 @@ class Stats(C.Structure):
 EXPORTS = [
     "b200ms_version", "b200ms_get_stats", "b200ms_default_options", "b200ms_create", "b200ms_destroy", "b200ms_set_options",
     "b200ms_last_error", "b200ms_host_alloc", "b200ms_host_free", "b200ms_solve_batch", "b200ms_bench_stencil", "b200ms_debug_schur", "b200ms_debug_setup",
-    "b200ms_debug_hierarchy", "b200ms_debug_batch", "b200ms_debug_apply", "b200ms_debug_vcycle", "b200ms_debug_solve", "b200ms_debug_march2_geometry", "b200ms_debug_post_tables", "b200ms_debug_post_tables_bounded", "b200ms_debug_te_terms", "b200ms_debug_grid_factors", "b200ms_debug_krylov",
+    "b200ms_debug_hierarchy", "b200ms_debug_batch", "b200ms_debug_apply", "b200ms_debug_vcycle", "b200ms_debug_solve", "b200ms_debug_march2_geometry", "b200ms_debug_post_tables", "b200ms_debug_post_tables_bounded", "b200ms_debug_te_terms", "b200ms_debug_grid_factors", "b200ms_debug_krylov", "b200ms_debug_fields",
 ]  # fmt: skip
 
 _lib = None
@@ -123,6 +123,7 @@ def lib():
             L.b200ms_debug_te_terms.argtypes = [_dp, C.c_int, C.c_int, C.c_double, C.c_double, C.c_int, C.c_int, _dp]
             L.b200ms_debug_grid_factors.argtypes = [C.POINTER(Problem), _dp, _dp, _dp]
             L.b200ms_debug_krylov.argtypes = [C.c_void_p, C.c_int, C.POINTER(Problem), C.c_int, C.c_int, C.c_int, _dp, _dp, _dp, _dp, _ip, _dp]
+            L.b200ms_debug_fields.argtypes = [C.c_void_p, C.c_int, C.POINTER(Problem), _dp, _dp, _ip, C.c_void_p]
             _lib = L
     return _lib
 

@@ -1771,7 +1771,87 @@ int krylov_run(b200ms_handle *h, const Window &W, int what, int prec, int nv, co
                                 ", nv " + std::to_string(nv) + ", restart " + std::to_string(S.restart) + ", m " + std::to_string(S.m) + ")";
   return rc;
 }
+
+// b200ms_debug_fields: caller vectors in the Ritz slots, then the solver's own epilogue (permutation and field recovery) into a
+// device buffer, copied back per problem
+template <typename T, typename C, typename P, typename PC>
+int fields_run(b200ms_handle *h, const Window &W, const b200ms_problem *probs, const double *vecs, const double *ncomplex, const int *perm,
+               void *out) {
+  const int B = W.i1 - W.i0;
+  std::vector<int> ids(B);
+  for (int b = 0; b < B; ++b) ids[b] = b;
+  std::vector<const ProblemSetup *> ps;
+  std::vector<MediumRef> refs;
+  const bool share = batch_refs(W, ids, ps, refs);
+  BatchSolver<T, C, P, PC> S(h->arena, h->stream, h->opt);
+  S.single_out_ = probs[0].precision == 1;
+  S.build(ps, share, upload_refs(h, refs, h->stream));
+  const int k = S.k;
+  std::vector<int> pm(perm, perm + (size_t)B * k);
+  for (int b = 0; b < B; ++b) {
+    std::vector<char> seen(k, 0);
+    for (int q = 0; q < k; ++q) {
+      const int s = pm[(size_t)b * k + q];
+      if (s < 0 || s >= k || seen[s]) {
+        h->err = "b200ms_debug_fields: perm of problem " + std::to_string(b) + " is not a permutation of 0.." + std::to_string(k - 1);
+        return B200MS_ERR_ARG;
+      }
+      seen[s] = 1;
+    }
+  }
+  const size_t n1 = (size_t)B * S.len;
+  std::vector<T> slot(n1);
+  for (int q = 0; q < k; ++q) {
+    for (size_t e = 0; e < n1; ++e) slot[e] = from_cd<T>(cd(vecs[2 * (q * n1 + e)], vecs[2 * (q * n1 + e) + 1]));
+    CUDA_CHECK(cudaMemcpyAsync(S.ritz_ptr() + (size_t)q * S.vstride, slot.data(), n1 * sizeof(T), cudaMemcpyHostToDevice, h->stream));
+    CUDA_CHECK(cudaStreamSynchronize(h->stream));
+  }
+  std::vector<cd> nsorted((size_t)B * k);
+  for (size_t i = 0; i < nsorted.size(); ++i) nsorted[i] = cd(ncomplex[2 * i], ncomplex[2 * i + 1]);
+  const size_t per = S.output_bytes_per_problem();
+  void *dev = nullptr;
+  CUDA_CHECK(cudaMalloc(&dev, per * B));
+  try {
+    CUDA_CHECK(cudaMemsetAsync(dev, 0xff, per * B, h->stream));  // NaN wherever the epilogue writes nothing
+    S.set_output(reinterpret_cast<cplx *>(dev));
+    S.epilogue(nsorted, pm, ps, nullptr, true);
+    CUDA_CHECK(cudaStreamSynchronize(h->stream));
+    CUDA_CHECK(cudaGetLastError());
+    CUDA_CHECK(cudaMemcpy(out, dev, per * B, cudaMemcpyDeviceToHost));
+  } catch (...) {
+    cudaFree(dev);
+    throw;
+  }
+  CUDA_CHECK(cudaFree(dev));
+  return B200MS_OK;
+}
 }  // namespace
+
+extern "C" int b200ms_debug_fields(b200ms_handle *h, int nprob, const b200ms_problem *probs, const double *vecs, const double *ncomplex,
+                                   const int *perm, void *out) {
+  if (!h || nprob < 1 || !probs || !vecs || !ncomplex || !perm || !out) return B200MS_ERR_ARG;
+  if (cudaSetDevice(h->device) != cudaSuccess) return B200MS_ERR_CUDA;
+  h->err.clear();
+  try {
+    Window W;
+    if (const int rc = debug_window(h, nprob, probs, "b200ms_debug_fields", W)) return rc;
+    const bool f32 = h->opt.mg_precision == 1;
+    switch (kind_of(W.setups[0])) {
+      case 0:
+        return f32 ? fields_run<double, double, float, float>(h, W, probs, vecs, ncomplex, perm, out)
+                   : fields_run<double, double, double, double>(h, W, probs, vecs, ncomplex, perm, out);
+      case 1:
+        return f32 ? fields_run<cplx, double, cplxf, float>(h, W, probs, vecs, ncomplex, perm, out)
+                   : fields_run<cplx, double, cplx, double>(h, W, probs, vecs, ncomplex, perm, out);
+      default:
+        return f32 ? fields_run<cplx, cplx, cplxf, cplxf>(h, W, probs, vecs, ncomplex, perm, out)
+                   : fields_run<cplx, cplx, cplx, cplx>(h, W, probs, vecs, ncomplex, perm, out);
+    }
+  } catch (const std::exception &e) {
+    h->err = e.what();
+    return B200MS_ERR_CUDA;
+  }
+}
 
 extern "C" int b200ms_debug_krylov(b200ms_handle *h, int nprob, const b200ms_problem *probs, int what, int prec, int nv, const double *V,
                                    const double *w, double *out, double *coef, int *iused, double *res) {
