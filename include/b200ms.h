@@ -29,7 +29,7 @@
 extern "C" {
 #endif
 
-#define B200MS_VERSION 209
+#define B200MS_VERSION 210
 
 /* return codes */
 enum {
@@ -96,6 +96,9 @@ typedef struct {
   /* ---- since version 206 ---- */
   const double *d2eps_table; /* NULL, or nmedia x 9 complex128 (re,im): d^2 eps / df^2 (1/Hz^2) of each medium at this problem's
                               frequency, rasterised like eps_table; only result.d2n_dfreq2 reads it (diagonal components) */
+  /* ---- since version 210 ---- */
+  const double *d3eps_table; /* NULL, or nmedia x 9 complex128 (re,im): d^3 eps / df^3 (1/Hz^3) of each medium at this problem's
+                              frequency, rasterised like eps_table; only result.d3n_dfreq3 reads it (diagonal components) */
 } b200ms_section;
 
 /* One eigenproblem == one compute_modes call (one plane, one frequency). */
@@ -145,6 +148,8 @@ typedef struct {
                             diagonal components are read, and only by the material term of result.dn_dfreq */
   const double *eps_d2freq; /* since version 206.  NULL, or d^2 eps_cross / df^2 (1/Hz^2) in the layout of `eps`; only the diagonal
                             components are read, and only by result.d2n_dfreq2 */
+  const double *eps_d3freq; /* since version 210.  NULL, or d^3 eps_cross / df^3 (1/Hz^3) in the layout of `eps`; only the diagonal
+                            components are read, and only by result.d3n_dfreq3 */
 } b200ms_problem;
 
 typedef struct {
@@ -204,6 +209,14 @@ typedef struct {
                             (1/Hz) of the caller's eps_cross at fixed d eps / df and PML stretch (0 at PEC-valued cells; NaN for a mode
                             whose correction solve stopped above 100 x inner_tol).  Gradient of the group index for a real change of
                             eps: Re dn_deps + f Re d2n_dfreq_deps.  HOST or DEVICE memory like `fields` */
+  /* ---- since version 210: third frequency derivative, from the correction solve of d2n_dfreq2 and the left correction of
+     d2n_dfreq_deps (no further solve; by the 2n+1 rule, see DESIGN.md §4):
+     lambda''' w^T v = w^T A'''v + 3 w_hat^T A''v + 3 w^T A''x + 6 w_hat^T A'x - 6 lambda' w_hat^T x - 3 lambda'' (w_hat^T v + w^T x)
+     in the scaled direction ' = f d/df.  Same scope as dn_dfreq; n_complex, the fields, dn_dfreq, dn_deps, d2n_dfreq2 and
+     d2n_dfreq_deps do not change when it is asked for ---- */
+  double *d3n_dfreq3;    /* NULL, or caller-allocated num_modes complex128 (re,im): d^3(n_eff + i k_eff)/df^3 (1/Hz^3), including the
+                            material dispersion of problem.eps_dfreq / eps_d2freq / eps_d3freq (section: deps_table / d2eps_table /
+                            d3eps_table).  NaN for a mode whose correction solve stopped above 100 x inner_tol */
 } b200ms_result;
 
 /* Tunables (all have defaults; see DESIGN.md). */

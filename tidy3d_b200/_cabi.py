@@ -17,7 +17,7 @@ import numpy as np
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("B200MS_LIB") or os.path.join(_HERE, "libb200ms.so")  # B200MS_LIB: developer override (A/B of builds)
 
-ABI_VERSION = 209  # B200MS_VERSION of include/b200ms.h
+ABI_VERSION = 210  # B200MS_VERSION of include/b200ms.h
 OK, ERR_SHAPE, ERR_NO_MODES, ERR_UNSUPPORTED, ERR_CUDA, ERR_NOCONV, ERR_ARG = range(7)
 SPEC_NAMES = {0: "diagonal", 1: "tensorial_real", 2: "tensorial_complex"}
 
@@ -28,7 +28,7 @@ _ip = C.POINTER(C.c_int)
 class SectionStruct(C.Structure):
     _fields_ = [("nrect", C.c_int), ("rects", _dp), ("medium", _ip), ("nmedia", C.c_int), ("eps_table", _dp),
                 ("shape", _ip), ("poly_start", _ip), ("poly_xy", _dp), ("site_medium", C.POINTER(C.c_ushort)), ("deps_table", _dp),
-                ("d2eps_table", _dp)]
+                ("d2eps_table", _dp), ("d3eps_table", _dp)]
 
 
 class Problem(C.Structure):
@@ -38,7 +38,7 @@ class Problem(C.Structure):
         ("freq", C.c_double), ("target_neff", C.c_double), ("bend_radius", C.c_double),
         ("angle_theta", C.c_double), ("angle_phi", C.c_double),
         ("eps", _dp), ("coords_x", _dp), ("coords_y", _dp), ("mu", _dp), ("section", C.POINTER(SectionStruct)), ("basis_e", _dp),
-        ("grid_correction", _dp), ("plane_bounds", _dp), ("eps_dfreq", _dp), ("eps_d2freq", _dp),
+        ("grid_correction", _dp), ("plane_bounds", _dp), ("eps_dfreq", _dp), ("eps_d2freq", _dp), ("eps_d3freq", _dp),
     ]  # fmt: skip
 
 
@@ -47,7 +47,7 @@ class Result(C.Structure):
         ("fields", _dp), ("n_complex", _dp), ("flux", _dp), ("te_fraction", _dp), ("overlap_prev", _dp), ("eps_spec", C.c_int), ("status", C.c_int), ("converged", C.c_int),
         ("outer_iters", C.c_int), ("op_applies", C.c_int), ("inner_iters", C.c_int), ("stencil_applies", C.c_int),
         ("is_complex", C.c_int), ("solve_ms", C.c_double), ("total_ms", C.c_double), ("max_residual", C.c_double),
-        ("dn_dfreq", _dp), ("dn_deps", _dp), ("d2n_dfreq2", _dp), ("d2n_residual", _dp), ("d2n_dfreq_deps", _dp),
+        ("dn_dfreq", _dp), ("dn_deps", _dp), ("d2n_dfreq2", _dp), ("d2n_residual", _dp), ("d2n_dfreq_deps", _dp), ("d3n_dfreq3", _dp),
     ]  # fmt: skip
 
 
@@ -137,11 +137,11 @@ class PackedProblem:
 
     def __init__(self, eps_cross, coords, freq, mode_spec, symmetry=(0, 0), direction="+", eps_packed=None, basis_fields=None,
                  mu_cross=None, target_override=None, incidence=False, post=0, section=None, grid_correction=None, plane_bounds=None,
-                 eps_dfreq=None, derivatives=False, eps_d2freq=None, second=False):
+                 eps_dfreq=None, derivatives=False, eps_d2freq=None, second=False, eps_d3freq=None, third=False):
         self.section = None
         if section is not None:  # geometric cross-section rasterised on the device (tidy3d_b200/sections.py); no eps array
             self.section, self._section_arrays = section.pack(float(freq), (len(coords[0]) - 1, len(coords[1]) - 1), dispersion=derivatives,
-                                                                  second=second)
+                                                                  second=second, third=third)
             eps = None
         elif eps_packed is not None:
             eps = eps_packed
@@ -247,6 +247,14 @@ class PackedProblem:
             if self.eps_d2freq.shape != (9, self.nx, self.ny):
                 raise ValueError("eps_d2freq must have the nine components and the shape of eps_cross")
             p.eps_d2freq = _ptr(self.eps_d2freq.view(np.float64))
+        self.eps_d3freq = None
+        if eps_d3freq is not None:  # d^3 eps_cross / df^3 in the eps layout (material term of the third derivative)
+            if section is not None:
+                raise ValueError("eps_d3freq belongs to an eps_cross problem; a section's media carry their own dispersion")
+            self.eps_d3freq = np.ascontiguousarray(np.stack([np.asarray(eps_d3freq[i], dtype=np.complex128) for i in range(len(eps_d3freq))]))
+            if self.eps_d3freq.shape != (9, self.nx, self.ny):
+                raise ValueError("eps_d3freq must have the nine components and the shape of eps_cross")
+            p.eps_d3freq = _ptr(self.eps_d3freq.view(np.float64))
         self.struct = p
         self.num_modes = p.num_modes
 
@@ -338,7 +346,7 @@ class Handle:
             pass
 
     def solve_batch(self, packed, want_fields=True, fields_ptrs=None, want_flux=False, want_overlaps=False, want_dfreq=False, want_deps=False,
-                    want_d2freq=False, want_group_eps=False):
+                    want_d2freq=False, want_group_eps=False, want_d3freq=False):
         """packed: list of PackedProblem.  Returns (rc, fields list | None, n_complex list, Result structs).
 
         ``fields_ptrs``: optional list of raw addresses (host or DEVICE memory, e.g. ``tensor.data_ptr()``) the library
@@ -346,13 +354,14 @@ class Handle:
         Fields are complex128, or complex64 for ``precision == "single"`` problems (solver.py:265-267).  ``want_dfreq`` /
         ``want_deps``: d n / df and d n / d eps of every mode (``last_dn_dfreq`` / ``last_dn_deps``); ``want_d2freq``: d^2 n / df^2 and
         the residual of its correction solve (``last_d2n_dfreq2`` / ``last_d2n_residual``); ``want_group_eps``: d(dn/df) / d eps of
-        every mode from that correction solve (``last_d2n_dfreq_deps``)."""
+        every mode from that correction solve (``last_d2n_dfreq_deps``); ``want_d3freq``: d^3 n / df^3 of every mode from the same
+        correction solve (``last_d3n_dfreq3``)."""
         n = len(packed)
         probs = (Problem * n)(*[p.struct for p in packed])
         results = (Result * n)()
         fields, ncs = [], []
         self.last_flux, self.last_te, self.last_overlaps, self.last_dn_dfreq, self.last_dn_deps = [], [], [], [], []
-        self.last_d2n_dfreq2, self.last_d2n_residual, self.last_d2n_dfreq_deps = [], [], []
+        self.last_d2n_dfreq2, self.last_d2n_residual, self.last_d2n_dfreq_deps, self.last_d3n_dfreq3 = [], [], [], []
         for i, p in enumerate(packed):
             nc = np.zeros(p.num_modes, dtype=np.complex128)
             ncs.append(nc)
@@ -375,6 +384,10 @@ class Handle:
                 d = np.zeros((3, p.nx, p.ny, p.num_modes), dtype=np.complex128)
                 self.last_d2n_dfreq_deps.append(d)
                 results[i].d2n_dfreq_deps = _ptr(d.view(np.float64))
+            if want_d3freq:
+                d = np.zeros(p.num_modes, dtype=np.complex128)
+                self.last_d3n_dfreq3.append(d)
+                results[i].d3n_dfreq3 = _ptr(d.view(np.float64))
             if want_flux:
                 fl, te = np.zeros(p.num_modes), np.zeros(p.num_modes)
                 self.last_flux.append(fl)

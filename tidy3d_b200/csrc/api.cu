@@ -870,8 +870,9 @@ void derivative_pass(b200ms_handle *h, BatchSolver<T, C, P, PC> &S, const std::v
 // result.d2n_dfreq2 and result.d2n_residual of the problems that ask for them.  Per mode slot q: the projected right-hand side
 // r = -Pi A'v, one correction solve (A - lambda_q) x = r by the eigen-solve's own inner solver (Krylov shift lambda_q of every
 // problem; the multigrid stays built for sigma) and a scan for w^T A'x.  With result.d2n_dfreq_deps, group_grad_kernel then
-// sums w_hat^T v and writes slot q of the map from the same x.  It writes its own buffers, the first two slots of the
-// outer Krylov basis and the inner solver's scratch -- nothing the fields, the post-processing or the warm start read.
+// sums w_hat^T v and writes slot q of the map from the same x; with result.d3n_dfreq3, third_scan_kernel sums the six
+// products of lambda''' from the same x.  It writes its own buffers, the first two slots of the outer Krylov basis and the
+// inner solver's scratch -- nothing the fields, the post-processing or the warm start read.
 template <typename T, typename C, typename P, typename PC>
 void dispersion_pass(b200ms_handle *h, BatchSolver<T, C, P, PC> &S, const std::vector<const ProblemSetup *> &ps, const std::vector<int> &ids,
                      const Window &W, const b200ms_problem *prob, b200ms_result *res, const std::vector<cd> &nsorted,
@@ -879,16 +880,24 @@ void dispersion_pass(b200ms_handle *h, BatchSolver<T, C, P, PC> &S, const std::v
   const int B = (int)ids.size(), k = S.k, nx = S.nx, ny = S.ny;
   const size_t N = (size_t)nx * ny;
   std::vector<char> skip(B);
-  bool any_mat = false, any_gmap = false;
+  bool any_mat = false, any_gmap = false, any_third = false;
   for (int b = 0; b < B; ++b) {
     const b200ms_problem &p = prob[W.i0 + ids[b]];
     const b200ms_result &rb = res[W.i0 + ids[b]];
-    skip[b] = (rb.d2n_dfreq2 || rb.d2n_dfreq_deps) ? 0 : 1;
+    skip[b] = (rb.d2n_dfreq2 || rb.d2n_dfreq_deps || rb.d3n_dfreq3) ? 0 : 1;
     any_gmap = any_gmap || rb.d2n_dfreq_deps;
+    any_third = any_third || rb.d3n_dfreq3;
     any_mat = any_mat || (p.eps ? (p.eps_dfreq || p.eps_d2freq) : (p.section->deps_table || p.section->d2eps_table));
   }
-  // host tables: f^2 d^2c/df^2 = 2 (f dc/df)^2 / c = 2 c (kappa / s)^2, frequencies
+  for (int b = 0; b < B && any_third; ++b) {  // the third-order terms also read eps'''
+    const b200ms_problem &p = prob[W.i0 + ids[b]];
+    any_mat = any_mat || (p.eps ? p.eps_d3freq != nullptr : p.section->d3eps_table != nullptr);
+  }
+  // host tables: f^2 d^2c/df^2 = 2 (f dc/df)^2 / c = 2 c (kappa / s)^2, frequencies; for the third-order pass
+  // f^3 d^3c/df^3 = -6 c (kappa / s)^3 and the combined directions c' +- c''
   std::vector<T> c2x((size_t)B * 4 * nx), c2y((size_t)B * 4 * ny);
+  const size_t n3x = any_third ? (size_t)B * 4 * nx : 0, n3y = any_third ? (size_t)B * 4 * ny : 0;
+  std::vector<T> c3x(n3x), c3y(n3y), csx(n3x), csy(n3y), cdx(n3x), cdy(n3y);
   std::vector<double> freq(B);
   for (int b = 0; b < B; ++b) {
     freq[b] = prob[W.i0 + ids[b]].freq;
@@ -905,22 +914,52 @@ void dispersion_pass(b200ms_handle *h, BatchSolver<T, C, P, PC> &S, const std::v
           c2[(size_t)w * n + i] = from_cd<T>(2.0 * c[(size_t)w * n + i] * r * r);
         }
       }
+      if (!any_third) continue;
+      const size_t o = (size_t)b * 4 * n;
+      for (int i = 0; i < n; ++i) {
+        const cd rf = A.lf[i].real() / A.lf[i], rb = A.lb[i].real() / A.lb[i];
+        for (int w = 0; w < 4; ++w) {
+          const cd r = w < 2 ? rf : rb, cw = c[(size_t)w * n + i];
+          const cd d1 = -cw * r, d2 = 2.0 * cw * r * r;
+          (a == 0 ? c3x : c3y)[o + (size_t)w * n + i] = from_cd<T>(-6.0 * cw * r * r * r);
+          (a == 0 ? csx : csy)[o + (size_t)w * n + i] = from_cd<T>(d1 + d2);
+          (a == 0 ? cdx : cdy)[o + (size_t)w * n + i] = from_cd<T>(d1 - d2);
+        }
+      }
     }
   }
   auto arr1 = [](const b200ms_problem &p) { return p.eps_dfreq; };
   auto tab1 = [](const b200ms_section &sec) { return sec.deps_table; };
   auto arr2 = [](const b200ms_problem &p) { return p.eps_d2freq; };
   auto tab2 = [](const b200ms_section &sec) { return sec.d2eps_table; };
+  auto arr3 = [](const b200ms_problem &p) { return p.eps_d3freq; };
+  auto tab3 = [](const b200ms_section &sec) { return sec.d3eps_table; };
   const int nch = (int)std::min<size_t>(kDerivChunks, (N + 255) / 256);
   const size_t o_c2x = 0, o_c2y = align256(c2x.size() * sizeof(T)), o_f = o_c2y + align256(c2y.size() * sizeof(T));
   const size_t o_part = o_f + align256(B * sizeof(double)), o_sum = o_part + align256((size_t)B * nch * 3 * sizeof(cplx));
   const size_t o_beta = o_sum + align256((size_t)B * 3 * sizeof(cplx)), o_p1 = o_beta + align256(B * sizeof(cplx));
   const size_t pbytes = any_mat ? align256((size_t)B * 3 * N * sizeof(cplx)) : 0, o_p2 = o_p1 + pbytes, o_sec = o_p2 + pbytes;
-  const size_t sec_bytes = any_mat ? std::max(gather_scratch_bytes(ids, W, prob, nx, ny, tab1), gather_scratch_bytes(ids, W, prob, nx, ny, tab2)) : 0;
+  size_t sec_bytes = any_mat ? std::max(gather_scratch_bytes(ids, W, prob, nx, ny, tab1), gather_scratch_bytes(ids, W, prob, nx, ny, tab2)) : 0;
+  if (any_mat && any_third) sec_bytes = std::max(sec_bytes, gather_scratch_bytes(ids, W, prob, nx, ny, tab3));
   // group-gradient pass: per-problem (alpha, beta), the sum w_hat^T v and the map [B][3][N][M]
   const size_t o_ab = align256(o_sec + sec_bytes), o_hsum = o_ab + align256((size_t)B * 2 * sizeof(cplx));
   const size_t o_gmap = o_hsum + align256((size_t)B * 3 * sizeof(cplx));
-  h->disp.reserve(any_gmap ? o_gmap + (size_t)B * 3 * N * k * sizeof(cplx) + 256 : o_sec + sec_bytes + 256);
+  size_t end = any_gmap ? o_gmap + align256((size_t)B * 3 * N * k * sizeof(cplx)) : align256(o_sec + sec_bytes);
+  // third-order pass: c''', c' + c'', c' - c'' per axis, p''', p' + p'', p' - p'', its partial sums and the six sums per problem
+  size_t o_c3[6] = {0, 0, 0, 0, 0, 0}, o_p3 = 0, o_tpart = 0, o_tsum = 0;
+  if (any_third) {
+    for (int e = 0; e < 6; ++e) {
+      o_c3[e] = end;
+      end += align256((e % 2 == 0 ? n3x : n3y) * sizeof(T));
+    }
+    o_p3 = end;
+    end += 3 * pbytes;
+    o_tpart = end;
+    end += align256((size_t)B * 2 * nch * 3 * sizeof(cplx));
+    o_tsum = end;
+    end += align256((size_t)B * 6 * sizeof(cplx));
+  }
+  h->disp.reserve(end + 256);
   unsigned char *base = h->disp.p;
   cudaStream_t st = h->stream;
   CUDA_CHECK(cudaMemcpyAsync(base + o_c2x, c2x.data(), c2x.size() * sizeof(T), cudaMemcpyHostToDevice, st));
@@ -935,8 +974,16 @@ void dispersion_pass(b200ms_handle *h, BatchSolver<T, C, P, PC> &S, const std::v
     cplx *p1 = reinterpret_cast<cplx *>(base + o_p1), *p2 = reinterpret_cast<cplx *>(base + o_p2);
     gather_diag(h, ids, W, prob, nx, ny, arr1, tab1, p1, base + o_sec);
     gather_diag(h, ids, W, prob, nx, ny, arr2, tab2, p2, base + o_sec);
+    cplx *p3 = nullptr, *pps = nullptr, *ppd = nullptr;
+    if (any_third) {
+      p3 = reinterpret_cast<cplx *>(base + o_p3);
+      pps = reinterpret_cast<cplx *>(base + o_p3 + pbytes);
+      ppd = reinterpret_cast<cplx *>(base + o_p3 + 2 * pbytes);
+      gather_diag(h, ids, W, prob, nx, ny, arr3, tab3, p3, base + o_sec);
+    }
     disp_fields_kernel<C><<<(unsigned)std::min<size_t>(((size_t)B * N + 255) / 256, 4096), 256, 0, st>>>(
-        nx, ny, B, da.fields, da.field_bstride, da.jz_e, da.jz_axis, da.jz_len, reinterpret_cast<const double *>(base + o_f), p1, p2);
+        nx, ny, B, da.fields, da.field_bstride, da.jz_e, da.jz_axis, da.jz_len, reinterpret_cast<const double *>(base + o_f), p1, p2, p3,
+        pps, ppd);
     CUDA_CHECK(cudaGetLastError());
     h->stats.launches += 1;
     a.p1 = p1;
@@ -948,6 +995,21 @@ void dispersion_pass(b200ms_handle *h, BatchSolver<T, C, P, PC> &S, const std::v
   T *r = S.basis0(), *x = S.basis0() + S.vstride;
   a.r = r;
   a.x = x;
+  ThirdArgs<T> ta{};
+  if (any_third) {
+    const std::vector<T> *tabs[6] = {&c3x, &c3y, &csx, &csy, &cdx, &cdy};
+    for (int e = 0; e < 6; ++e)
+      CUDA_CHECK(cudaMemcpyAsync(base + o_c3[e], tabs[e]->data(), tabs[e]->size() * sizeof(T), cudaMemcpyHostToDevice, st));
+    ta.c3x = reinterpret_cast<const T *>(base + o_c3[0]); ta.c3y = reinterpret_cast<const T *>(base + o_c3[1]);
+    ta.csx = reinterpret_cast<const T *>(base + o_c3[2]); ta.csy = reinterpret_cast<const T *>(base + o_c3[3]);
+    ta.cdx = reinterpret_cast<const T *>(base + o_c3[4]); ta.cdy = reinterpret_cast<const T *>(base + o_c3[5]);
+    if (a.p1) {
+      ta.p3 = reinterpret_cast<const cplx *>(base + o_p3);
+      ta.ps = reinterpret_cast<const cplx *>(base + o_p3 + pbytes);
+      ta.pd = reinterpret_cast<const cplx *>(base + o_p3 + 2 * pbytes);
+    }
+    ta.partial = reinterpret_cast<cplx *>(base + o_tpart);
+  }
   auto scan = [&](int phase, std::vector<cplx> &sums) {
     const dim3 g(phase == 1 ? (unsigned)std::min<size_t>((N + 255) / 256, 1024) : (unsigned)nch, B);
     if (S.has_mu) disp_scan_kernel<T, C, true><<<g, 256, 0, st>>>(a, phase);
@@ -1028,6 +1090,36 @@ void dispersion_pass(b200ms_handle *h, BatchSolver<T, C, P, PC> &S, const std::v
       else group_grad_kernel<T, C, false><<<grd, blk, 0, st>>>(a, 1, dab, gmap);
       CUDA_CHECK(cudaGetLastError());
       h->stats.launches += 3;
+    }
+    if (any_third) {  // lambda''' of slot q from the same x (third_scan_kernel)
+      const dim3 g0(nch, B);
+      cplx *tsum = reinterpret_cast<cplx *>(base + o_tsum);
+      if (S.has_mu) third_scan_kernel<T, C, true><<<g0, 256, 0, st>>>(a, ta);
+      else third_scan_kernel<T, C, false><<<g0, 256, 0, st>>>(a, ta);
+      deriv_final_kernel<<<(B * 6 + 127) / 128, 128, 0, st>>>(ta.partial, nch, B * 6, tsum);
+      CUDA_CHECK(cudaGetLastError());
+      h->stats.launches += 2;
+      std::vector<cplx> s3((size_t)B * 6);
+      CUDA_CHECK(cudaMemcpyAsync(s3.data(), tsum, s3.size() * sizeof(cplx), cudaMemcpyDeviceToHost, st));
+      CUDA_CHECK(cudaStreamSynchronize(st));
+      for (int b = 0; b < B; ++b) {
+        b200ms_result &rr = res[W.i0 + ids[b]];
+        if (skip[b] || !rr.d3n_dfreq3) continue;
+        const cplx *s = sv.data() + (size_t)b * 3, *t = sx.data() + (size_t)b * 3, *u = s3.data() + (size_t)b * 6;
+        auto zc = [](const cplx &z) { return cd(z.re, z.im); };
+        const cd wv = zc(s[0]), l1 = zc(s[1]) / wv, wx = zc(t[0]);
+        const cd l2 = (zc(s[2]) + 2.0 * (zc(t[1]) - l1 * wx)) / wv;
+        const cd hv = zc(u[0]), hx = zc(u[1]), w3v = zc(u[2]), h2v = zc(u[3]), w2x = zc(u[4]), h1x = zc(u[5]);
+        const cd l3 = (w3v + 3.0 * h2v + 3.0 * w2x + 6.0 * h1x - 6.0 * l1 * hx - 3.0 * l2 * (hv + wx)) / wv;  // f^3 d^3 lambda / df^3
+        const double f = freq[b];
+        const cd dl = l1 / f, d2l = l2 / (f * f), d3l = l3 / (f * f * f);
+        const cd sn = nsorted[(size_t)b * k + q];
+        const cd ds = -dl / (2.0 * sn), d2s = -(d2l + 2.0 * ds * ds) / (2.0 * sn), d3s = -(d3l + 6.0 * ds * d2s) / (2.0 * sn);
+        cd d3n = ps[b]->knorm * d3s;
+        if (std::abs(wv) == 0 || !(resv[b] <= 100.0 * tol)) d3n = cd(std::nan(""), std::nan(""));
+        rr.d3n_dfreq3[2 * q] = d3n.real();
+        rr.d3n_dfreq3[2 * q + 1] = d3n.imag();
+      }
     }
   }
   S.reset_sigma();
@@ -1141,8 +1233,8 @@ void solve_group(b200ms_handle *h, const std::vector<int> &ids, const Window &W,
   bool want_deriv = false, want_disp = false;
   for (int b = 0; b < B; ++b) {
     const b200ms_result &rb = res[W.i0 + ids[b]];
-    want_deriv = want_deriv || rb.dn_dfreq || rb.dn_deps || rb.d2n_dfreq2 || rb.d2n_dfreq_deps;
-    want_disp = want_disp || rb.d2n_dfreq2 || rb.d2n_dfreq_deps;
+    want_deriv = want_deriv || rb.dn_dfreq || rb.dn_deps || rb.d2n_dfreq2 || rb.d2n_dfreq_deps || rb.d3n_dfreq3;
+    want_disp = want_disp || rb.d2n_dfreq2 || rb.d2n_dfreq_deps || rb.d3n_dfreq3;
   }
   if (want_deriv) {
     DerivArgs<T, C> da;
@@ -1283,7 +1375,7 @@ extern "C" int b200ms_solve_batch(b200ms_handle *h, int nprob, const b200ms_prob
           res[i].eps_spec = s.eps_spec;
           res[i].is_complex = s.is_complex;
           std::string err = s.error;
-          if (res[i].status == B200MS_OK && (res[i].dn_dfreq || res[i].dn_deps || res[i].d2n_dfreq2 || res[i].d2n_dfreq_deps) && (s.tensorial || s.relative || s.masked)) {
+          if (res[i].status == B200MS_OK && (res[i].dn_dfreq || res[i].dn_deps || res[i].d2n_dfreq2 || res[i].d2n_dfreq_deps || res[i].d3n_dfreq3) && (s.tensorial || s.relative || s.masked)) {
             res[i].status = B200MS_ERR_UNSUPPORTED;
             err = s.tensorial ? "mode derivatives: tensorial problems (angled planes, off-diagonal eps) are not supported"
                   : s.relative ? "mode derivatives: the relative mode solver (basis fields) is not supported"

@@ -314,9 +314,11 @@ __global__ void __launch_bounds__(256) disp_scan_kernel(DispArgs<T, C> a, int ph
 // [B][3][N] f dp/df and f^2 d^2p/df^2 of p = (exx, eyy, iez) in the solver frame from d eps / df and d^2 eps / df^2 of the caller's
 // diagonal (in place: dp1 holds d eps / df on entry, dp2 d^2 eps / df^2).  Bend: exx = eps_xx / je, eyy = eps_yy / je,
 // ezz = je eps_zz; freq: [B] Hz.  iez' = -ezz' iez^2, iez'' = 2 ezz'^2 iez^3 - ezz'' iez^2.  PEC-valued cells: 0 (as eps_grad).
+// With dp3 (the third-order pass): dp3 holds d^3 eps / df^3 on entry and receives f^3 d^3p/df^3, iez''' = -ezz''' iez^2 +
+// 6 ezz' ezz'' iez^3 - 6 ezz'^3 iez^4, and dps / dpd receive the combined directions p' + p'' and p' - p''.
 template <typename C>
 __global__ void disp_fields_kernel(int nx, int ny, int B, const C *fields, size_t field_bstride, const double *jz_e, int jz_axis, int jz_len,
-                                   const double *freq, cplx *dp1, cplx *dp2) {
+                                   const double *freq, cplx *dp1, cplx *dp2, cplx *dp3, cplx *dps, cplx *dpd) {
   const size_t N = (size_t)nx * ny;
   for (size_t t = (size_t)blockIdx.x * blockDim.x + threadIdx.x; t < (size_t)B * N; t += (size_t)gridDim.x * blockDim.x) {
     const int b = (int)(t / N);
@@ -338,6 +340,18 @@ __global__ void disp_fields_kernel(int nx, int ny, int B, const C *fields, size_
     const cplx iz2 = iz * iz;
     d1[2 * N] = is_pec ? mk(0.0, 0.0) : -(e1 * iz2);
     d2[2 * N] = is_pec ? mk(0.0, 0.0) : 2.0 * (e1 * e1) * (iz2 * iz) - e2 * iz2;
+    if (!dp3) continue;
+    cplx *d3 = dp3 + (size_t)b * 3 * N + g, *ds = dps + (size_t)b * 3 * N + g, *dd = dpd + (size_t)b * 3 * N + g;
+    for (int k = 0; k < 2; ++k) {
+      const bool pk = abs2(to_cplx(ldg(fb + (size_t)k * N + g))) >= pec * pec;
+      d3[(size_t)k * N] = pk ? mk(0.0, 0.0) : d3[(size_t)k * N] * (f * f * f / je);
+    }
+    const cplx e3 = d3[2 * N] * (f * f * f * je);  // f^3 ezz'''
+    d3[2 * N] = is_pec ? mk(0.0, 0.0) : 6.0 * (e1 * e2) * (iz2 * iz) - e3 * iz2 - 6.0 * (e1 * e1 * e1) * (iz2 * iz2);
+    for (int k = 0; k < 3; ++k) {
+      ds[(size_t)k * N] = d1[(size_t)k * N] + d2[(size_t)k * N];
+      dd[(size_t)k * N] = d1[(size_t)k * N] - d2[(size_t)k * N];
+    }
   }
 }
 
@@ -529,6 +543,130 @@ __global__ void __launch_bounds__(256) group_grad_kernel(DispArgs<T, C> a, int m
     if (is_pec[k]) num = g0 = mk(0.0, 0.0);
     o[((size_t)k * N + g) * M + a.q] = al * num + be * g0;
   }
+}
+
+// ------------------------------------------------------------------------------------------------
+// Third-order pass: the third frequency derivative of lambda from the dispersion pass's correction x and the left correction
+// w_hat of the group-gradient pass (oracle/mode_third_order.py is the float64 model).  By Wigner's 2n+1 rule,
+//   lambda''' w^T v = w^T A'''v + 3 w_hat^T A''v + 3 w^T A''x + 6 w_hat^T A'x - 6 lambda' w_hat^T x - 3 lambda'' (w_hat^T v + w^T x)
+// needs no further solve.  A has bidegree (2, 2) in (c, p), so with E(a, b) = A(c + a, p + b) v the terms of A'''v are exact
+// with unit steps: A_c[c'''] = [E(c''') - E(-c''')]/2, 3 A_cc[c', c''] = 3/4 [E(c'+c'') - E(c'-c'') - E(-c'+c'') + E(-c'-c'')]
+// (A_p, A_pp alike), 3 A_cp[a, b] = 3/4 [E(a, b) - E(a, -b) - E(-a, b) + E(-a, -b)] for (c', p'') and (c'', p'), and
+// 3 A_ccp[c', c', p'] + 3 A_cpp[c', p', p'] = 3 [E(c', p') - E(-c', -p') - E(0, p') + E(0, -p') - E(c', 0) + E(-c', 0)].
+// Per mode slot one scan sums, per problem, (w_hat^T v, w_hat^T x, w^T A'''v) and (w_hat^T A''v, w^T A''x, w_hat^T A'x).
+// ------------------------------------------------------------------------------------------------
+
+// one operator evaluation of A'''v: coefficient direction (0 none, 1 c', 2 c'', 3 c''', 4 c' + c'', 5 c' - c'') and step, field
+// direction (0 none, 1 p', 2 p'', 3 p''', 4 p' + p'', 5 p' - p'') and step, weight.  The first six move only the coefficients.
+struct ThirdTerm {
+  int cdir, pdir;
+  double sc, sp, w;
+};
+__constant__ ThirdTerm kThirdTerms[26] = {
+    {3, 0, 1.0, 0.0, 0.5},    {3, 0, -1.0, 0.0, -0.5},  {4, 0, 1.0, 0.0, 0.75},   {5, 0, 1.0, 0.0, -0.75},  {5, 0, -1.0, 0.0, -0.75},
+    {4, 0, -1.0, 0.0, 0.75},  {0, 3, 0.0, 1.0, 0.5},    {0, 3, 0.0, -1.0, -0.5},  {0, 4, 0.0, 1.0, 0.75},   {0, 5, 0.0, 1.0, -0.75},
+    {0, 5, 0.0, -1.0, -0.75}, {0, 4, 0.0, -1.0, 0.75},  {1, 2, 1.0, 1.0, 0.75},   {1, 2, 1.0, -1.0, -0.75}, {1, 2, -1.0, 1.0, -0.75},
+    {1, 2, -1.0, -1.0, 0.75}, {2, 1, 1.0, 1.0, 0.75},   {2, 1, 1.0, -1.0, -0.75}, {2, 1, -1.0, 1.0, -0.75}, {2, 1, -1.0, -1.0, 0.75},
+    {1, 1, 1.0, 1.0, 3.0},    {1, 1, -1.0, -1.0, -3.0}, {0, 1, 0.0, 1.0, -3.0},   {0, 1, 0.0, -1.0, 3.0},   {1, 0, 1.0, 0.0, -3.0},
+    {1, 0, -1.0, 0.0, 3.0}};
+
+template <typename T>
+struct ThirdArgs {
+  const T *c3x, *c3y;        // [B][4][n] f^3 d^3c/df^3 = 6 c'^3 / c^2
+  const T *csx, *csy;        // [B][4][n] c' + c''
+  const T *cdx, *cdy;        // [B][4][n] c' - c''
+  const cplx *p3, *ps, *pd;  // [B][3][N] p''', p' + p'', p' - p'' (null with a nondispersive batch)
+  cplx *partial;             // [B][2][nchunk][3]
+};
+
+// grid (nchunk, B), 256 threads, one mode slot a.q while a.x holds its correction (see above)
+template <typename T, typename C, bool HAS_MU>
+__global__ void __launch_bounds__(256) third_scan_kernel(DispArgs<T, C> a, ThirdArgs<T> t) {
+  const DerivArgs<T, C> &d = a.d;
+  const int b = blockIdx.y, nx = d.nx, ny = d.ny;
+  const size_t N = (size_t)nx * ny;
+  const bool hp = a.p1 != nullptr;
+  const DispTerm *tab2 = hp ? kDispTermsP : kDispTermsC;
+  const int n2 = hp ? 13 : 5, n3 = hp ? 26 : 6;
+  const T *vb = d.vec + (size_t)a.q * d.vstride + (size_t)b * 2 * N, *xb = a.x + (size_t)b * 2 * N;
+  const size_t o4x = (size_t)b * 4 * nx, o4y = (size_t)b * 4 * ny, o3 = (size_t)b * 3 * N;
+  const GroupCell<T, C, HAS_MU> G{vb, xb, d.fields + d.field_bstride * b, d.cx + o4x, d.cy + o4y, d.dcx + o4x, d.dcy + o4y,
+                                  d.gx + (size_t)b * 2 * nx, d.gy + (size_t)b * 2 * ny, hp ? a.p1 + o3 : nullptr, nx, ny, N};
+  const T *cxb = d.cx + o4x, *cyb = d.cy + o4y;
+  // direction k of the coefficients (per axis) and of the fields, selected per term (a table of pointers would stay in registers)
+  auto rows = [&](int k, int ax) -> const T * {
+    const size_t o = ax == 0 ? o4x : o4y;
+    switch (k) {
+      case 1: return (ax == 0 ? d.dcx : d.dcy) + o;
+      case 2: return (ax == 0 ? a.c2x : a.c2y) + o;
+      case 3: return (ax == 0 ? t.c3x : t.c3y) + o;
+      case 4: return (ax == 0 ? t.csx : t.csy) + o;
+      case 5: return (ax == 0 ? t.cdx : t.cdy) + o;
+      default: return nullptr;
+    }
+  };
+  auto fdir = [&](int k) -> const cplx * {
+    if (!hp) return nullptr;
+    switch (k) {
+      case 1: return a.p1 + o3;
+      case 2: return a.p2 + o3;
+      case 3: return t.p3 + o3;
+      case 4: return t.ps + o3;
+      case 5: return t.pd + o3;
+      default: return nullptr;
+    }
+  };
+  const C *fb = d.fields + d.field_bstride * b;
+  cplx s[6] = {mk(0.0, 0.0), mk(0.0, 0.0), mk(0.0, 0.0), mk(0.0, 0.0), mk(0.0, 0.0), mk(0.0, 0.0)};
+  for (size_t g = (size_t)blockIdx.x * 256 + threadIdx.x; g < N; g += (size_t)gridDim.x * 256) {
+    const int i = (int)(g / ny), j = (int)(g % ny);
+    cplx a2v[2] = {mk(0.0, 0.0), mk(0.0, 0.0)}, a2x[2] = {mk(0.0, 0.0), mk(0.0, 0.0)}, a1x[2] = {mk(0.0, 0.0), mk(0.0, 0.0)};
+#pragma unroll 1
+    for (int k = 0; k < n2; ++k) {  // A'' on v and on x, A' on x
+      const DispTerm tm = tab2[k];
+      const CoefRows<T> CX{cxb, rows(tm.cdir, 0), tm.sc, nx}, CY{cyb, rows(tm.cdir, 1), tm.sc, ny};
+      const cplx *dp = fdir(tm.pdir);
+      const PertSite<T, C, HAS_MU> Pv{vb, vb + N, fb, dp, tm.sp, CX, CY, nx, ny, N};
+      const PertSite<T, C, HAS_MU> Px{xb, xb + N, fb, dp, tm.sp, CX, CY, nx, ny, N};
+      cplx y1, y2;
+      Pv.apply(i, j, y1, y2);
+      a2v[0] += tm.w2 * y1;
+      a2v[1] += tm.w2 * y2;
+      Px.apply(i, j, y1, y2);
+      a2x[0] += tm.w2 * y1;
+      a2x[1] += tm.w2 * y2;
+      a1x[0] += tm.w1 * y1;
+      a1x[1] += tm.w1 * y2;
+    }
+    cplx a3v[2] = {mk(0.0, 0.0), mk(0.0, 0.0)};
+#pragma unroll 1
+    for (int k = 0; k < n3; ++k) {  // A''' on v
+      const ThirdTerm tm = kThirdTerms[k];
+      const PertSite<T, C, HAS_MU> Pv{vb, vb + N, fb, fdir(tm.pdir), tm.sp, CoefRows<T>{cxb, rows(tm.cdir, 0), tm.sc, nx},
+                                      CoefRows<T>{cyb, rows(tm.cdir, 1), tm.sc, ny}, nx, ny, N};
+      cplx y1, y2;
+      Pv.apply(i, j, y1, y2);
+      a3v[0] += tm.w * y1;
+      a3v[1] += tm.w * y2;
+    }
+    cplx w[2], h[2];  // w and w_hat at (i, j), formed after the operator terms so that they do not hold registers through them
+    G.ww(i, j, w, h);
+    s[0] += h[0] * to_cplx(ldg(vb + g)) + h[1] * to_cplx(ldg(vb + N + g));
+    s[1] += h[0] * to_cplx(ldg(xb + g)) + h[1] * to_cplx(ldg(xb + N + g));
+    s[2] += w[0] * a3v[0] + w[1] * a3v[1];
+    s[3] += h[0] * a2v[0] + h[1] * a2v[1];
+    s[4] += w[0] * a2x[0] + w[1] * a2x[1];
+    s[5] += h[0] * a1x[0] + h[1] * a1x[1];
+  }
+  __shared__ cplx red[6][256];
+  for (int k = 0; k < 6; ++k) red[k][threadIdx.x] = s[k];
+  __syncthreads();
+  for (int hh = 128; hh > 0; hh >>= 1) {
+    if ((int)threadIdx.x < hh)
+      for (int k = 0; k < 6; ++k) red[k][threadIdx.x] += red[k][threadIdx.x + hh];
+    __syncthreads();
+  }
+  if (threadIdx.x < 6) t.partial[(((size_t)b * 2 + threadIdx.x / 3) * gridDim.x + blockIdx.x) * 3 + threadIdx.x % 3] = red[threadIdx.x][0];
 }
 
 }  // namespace b200ms

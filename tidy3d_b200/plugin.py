@@ -232,3 +232,21 @@ def dispersion_of(freq, dn_dfreq, d2n_dfreq2):
     the three-point formula of ``group_index``.  ``freq`` broadcasts against the derivatives (e.g. shape (F, 1) with (F, M))."""
     f = np.asarray(freq, float)
     return -1e18 * f**2 * (2 * np.real(dn_dfreq) + f * np.real(d2n_dfreq2)) / C0_UM**2
+
+
+def dispersion_slope_of(freq, dn_dfreq, d2n_dfreq2, d3n_dfreq3):
+    """Dispersion slope S = dD / d(wavelength) (ps/(nm^2 km)) from analytic frequency derivatives of n_eff + i k_eff
+    (``compute_modes_batch(..., derivatives=("freq3",))``): dD/df = -1e18 (4 f Re n' + 5 f^2 Re n'' + f^3 Re n''') / c0^2 (c0 in
+    um/s) and S = -(f^2 / c) dD/df with c in nm/s, the step -> 0 limit of a central difference of ``dispersion_of`` over
+    wavelength.  ``freq`` broadcasts against the derivatives like in ``dispersion_of``."""
+    f = np.asarray(freq, float)
+    dd = -1e18 * (4 * f * np.real(dn_dfreq) + 5 * f**2 * np.real(d2n_dfreq2) + f**3 * np.real(d3n_dfreq3)) / C0_UM**2
+    return -(f**2 / (C0_UM * 1e3)) * dd
+
+
+def beta3_of(freq, d2n_dfreq2, d3n_dfreq3):
+    """Third-order dispersion beta3 = d^3 beta / d omega^3 (ps^3/km) of beta = omega n / c, from analytic frequency derivatives
+    of n_eff + i k_eff: beta3 = (3 Re n'' + f Re n''') / (4 pi^2 c), c in m/s (1 s^3/m = 1e39 ps^3/km).  ``freq`` broadcasts
+    against the derivatives like in ``dispersion_of``."""
+    f = np.asarray(freq, float)
+    return (3 * np.real(d2n_dfreq2) + f * np.real(d3n_dfreq3)) / (4 * np.pi**2 * (C0_UM * 1e-6)) * 1e39

@@ -99,6 +99,16 @@ class Medium:
         h = 1e-3 * freq
         return (self.tensor(freq + h) - 2 * self.tensor(freq) + self.tensor(freq - h)) / (h * h)
 
+    def d3tensor_dfreq3(self, freq: float) -> np.ndarray:
+        """d^3 eps / df^3 (1/Hz^3) of the 3x3 tensor: zero for a constant medium, a third central difference of ``eps(f)`` at
+        f +- h, f +- 2h for a dispersive one.  The relative step is 1e-3: the roundoff grows like eps_mach / step^3 (about 1e-7
+        relative to eps at 1e-3), the truncation error like step^2 (exact for a cubic eps(f))."""
+        if not callable(self.eps):
+            return np.zeros((3, 3), dtype=complex)
+        h = 1e-3 * freq
+        t = self.tensor
+        return (t(freq + 2 * h) - 2 * t(freq + h) + 2 * t(freq - h) - t(freq - 2 * h)) / (2 * h**3)
+
 
 def site_medium_from_masks(shape: Tuple[int, int], masks: Sequence[Tuple[np.ndarray, int]]) -> np.ndarray:
     """(3, Nx, Ny) uint16 site map from per-structure inside-masks, drawn in structure order like epsilon_on_grid
@@ -160,11 +170,13 @@ class Section:
             raise ValueError("Mismatch between 'coords' and 'site_medium' shapes.")
         return sm
 
-    def pack(self, freq: float, shape: Optional[Tuple[int, int]] = None, dispersion: bool = False, second: bool = False):
+    def pack(self, freq: float, shape: Optional[Tuple[int, int]] = None, dispersion: bool = False, second: bool = False,
+             third: bool = False):
         """ctypes ``b200ms_section`` for one frequency plus the arrays it points to (kept alive by the caller).  ``shape`` =
         (Nx, Ny) of the plane, needed to check ``site_medium``.  ``dispersion``: also pass every medium's d eps / df
         (``deps_table``), the material term of the mode derivatives; ``second``: also every medium's d^2 eps / df^2
-        (``d2eps_table``), the material term of the second frequency derivative."""
+        (``d2eps_table``), the material term of the second frequency derivative; ``third``: also every medium's d^3 eps / df^3
+        (``d3eps_table``), the material term of the third frequency derivative."""
         media, ids = self._media()
         n = len(self.structures)
         rects = np.zeros((n, 4), dtype=np.float64)
@@ -215,4 +227,8 @@ class Section:
         if second and any(callable(m.eps) for m in media):
             d2table = np.ascontiguousarray([m.d2tensor_dfreq2(freq).ravel() for m in media], dtype=np.complex128)
             st.d2eps_table = d2table.view(np.float64).ctypes.data_as(_cabi._dp)
-        return st, (rects, med, table, kinds, pstart, pxy, site, dtable, d2table)
+        d3table = None
+        if third and any(callable(m.eps) for m in media):
+            d3table = np.ascontiguousarray([m.d3tensor_dfreq3(freq).ravel() for m in media], dtype=np.complex128)
+            st.d3eps_table = d3table.view(np.float64).ctypes.data_as(_cabi._dp)
+        return st, (rects, med, table, kinds, pstart, pxy, site, dtable, d2table, d3table)

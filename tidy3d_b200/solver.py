@@ -113,19 +113,26 @@ def compute_modes_batch(
     permittivity gradient of the group index from the same correction solves (no further solve): ``d2n_dfreq_deps`` (3, Nx, Ny, M),
     d(dn/df) / d eps_{xx,yy,zz} (1/Hz) at every Yee site at fixed d eps / df and PML stretch (NaN where ``d2n_dfreq2`` is), and
     ``dng_deps`` = Re ``dn_deps`` + f Re ``d2n_dfreq_deps``, the gradient of ``n_group`` for a real change of eps.  It implies
-    ``"freq"``, ``"eps"`` and ``"freq2"``, whose outputs do not change.
+    ``"freq"``, ``"eps"`` and ``"freq2"``, whose outputs do not change.  ``"freq3"`` adds the third-order dispersion from the same
+    correction solves (no further solve, by the 2n+1 rule): ``d3n_dfreq3`` (d^3(n_eff + i k_eff)/df^3, 1/Hz^3; NaN where
+    ``d2n_dfreq2`` is), ``dispersion_slope`` (dD/d(wavelength), ps/(nm^2 km), ``plugin.dispersion_slope_of``) and ``beta3``
+    (d^3 beta / d omega^3, ps^3/km, ``plugin.beta3_of``).  It implies ``"freq2"`` and ``"freq"``, whose outputs do not change;
+    its material term also reads a problem's ``eps_d3freq=`` (d^3 eps_cross / df^3) or a section's callable media.
     """
     post = tuple(post or ())
     unknown = set(post) - {"gauge", "normalize", "flux", "overlaps"}
     if unknown:
         raise ValueError(f"unknown post-processing step(s): {sorted(unknown)}")
     derivatives = tuple(derivatives or ())
-    unknown = set(derivatives) - {"freq", "eps", "freq2", "group_eps"}
+    unknown = set(derivatives) - {"freq", "eps", "freq2", "group_eps", "freq3"}
     if unknown:
         raise ValueError(f"unknown derivative(s): {sorted(unknown)}")
     group_eps = "group_eps" in derivatives
     if group_eps:
         derivatives = derivatives + tuple(d for d in ("eps", "freq2") if d not in derivatives)
+    third = "freq3" in derivatives
+    if third and "freq2" not in derivatives:
+        derivatives = derivatives + ("freq2",)
     second = "freq2" in derivatives
     if second and "freq" not in derivatives:
         derivatives = derivatives + ("freq",)
@@ -154,6 +161,7 @@ def compute_modes_batch(
             incidence=(split is not None or p.get("mu_cross") is not None),  # solver.py:93
             post=post_flags, grid_correction=p.get("grid_correction"), plane_bounds=p.get("plane_bounds"),
             eps_dfreq=p.get("eps_dfreq"), derivatives="freq" in derivatives, eps_d2freq=p.get("eps_d2freq"), second=second,
+            eps_d3freq=p.get("eps_d3freq"), third=third,
         )  # fmt: skip
         if split is None and section is None:
             cache[key] = pk.eps
@@ -166,13 +174,15 @@ def compute_modes_batch(
         packed.append(pk)
     h = handle or get_handle(device)  # after input validation: argument errors do not need a GPU
     with h.lock:
-        dkw = dict(want_dfreq="freq" in derivatives, want_deps="eps" in derivatives, want_d2freq=second, want_group_eps=group_eps) if derivatives else {}
+        dkw = dict(want_dfreq="freq" in derivatives, want_deps="eps" in derivatives, want_d2freq=second, want_group_eps=group_eps,
+                   want_d3freq=third) if derivatives else {}
         rc, fields, ncs, results = h.solve_batch(packed, want_fields, fields_ptrs, want_flux=("flux" in post or "normalize" in post),
                                                  want_overlaps="overlaps" in post, **dkw)
         flux_out, te_out, ov_out = h.last_flux, h.last_te, h.last_overlaps
         dfreq_out, deps_out = (h.last_dn_dfreq, h.last_dn_deps) if derivatives else ([], [])
         d2_out, d2res_out = (h.last_d2n_dfreq2, h.last_d2n_residual) if second else ([], [])
         gmap_out = h.last_d2n_dfreq_deps if group_eps else []
+        d3_out = h.last_d3n_dfreq3 if third else []
         err = h.last_error() if rc != _cabi.OK else ""
     if rc != _cabi.OK:
         bad = [i for i in range(len(packed)) if results[i].status != _cabi.OK]
@@ -208,6 +218,13 @@ def compute_modes_batch(
         if gmap_out:
             infos[-1]["d2n_dfreq_deps"] = gmap_out[i]
             infos[-1]["dng_deps"] = deps_out[i].real + float(packed[i].struct.freq) * gmap_out[i].real
+        if d3_out:
+            from .plugin import beta3_of, dispersion_slope_of  # noqa: PLC0415  (plugin imports this module)
+
+            fq = float(packed[i].struct.freq)
+            infos[-1]["d3n_dfreq3"] = d3_out[i]
+            infos[-1]["dispersion_slope"] = dispersion_slope_of(fq, dfreq_out[i], d2_out[i], d3_out[i])
+            infos[-1]["beta3"] = beta3_of(fq, d2_out[i], d3_out[i])
     return (out, infos) if return_info else out
 
 
