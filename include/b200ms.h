@@ -378,7 +378,13 @@ int b200ms_debug_post_tables_bounded(const double *coords, int n, int sym, doubl
  *           *iters (when not NULL) gets a bit mask of the levels whose residual was restricted inside the residual kernel
  *           (transfer_vec bit 2).
  *   what 2: out = (A - sigma)^-1 in by the inner solver of the eigen-iteration, to the handle's inner_tol; *iters gets its
- *           Arnoldi steps, relres[nprob] the final relative residual of every problem. */
+ *           Arnoldi steps, relres[nprob] the final relative residual of every problem.
+ *   Tensorial problems only (else B200MS_ERR_ARG), level 0; these two modes change no struct, so they carry no version of their
+ *   own: a library without them returns B200MS_ERR_ARG for what > 2.
+ *   what 3: the transposed Krylov-side operator, out = (A^T - sigma) in  /  in2 - (A^T - sigma) in  for mode 0 / 1, with A the
+ *           4N first-order operator msign (-i) M (the operator whose eigenvectors are the left eigenvectors of A).
+ *   what 4: one application of the transposed block preconditioner, out ~ (A_d^T - sigma)^-1 in, A_d the diagonal-tensor part:
+ *           -K (A_d + sigma)^-1 K^-1 through the local pairing K A_d = -A_d^T K (oracle/tensor_derivatives.py). */
 int b200ms_debug_batch(b200ms_handle *h, int nprob, const b200ms_problem *probs, int what, int level, int mode,
                        const double *in, const double *in2, double *out, int *iters, double *relres);
 /* b200ms_debug_batch with one problem: apply (what 0), V-cycle (what 1), inner solve (what 2) */

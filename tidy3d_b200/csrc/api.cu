@@ -1755,6 +1755,14 @@ int debug_run(b200ms_handle *h, const Window &W, int what, int level, int mode, 
   std::vector<MediumRef> refs;
   const bool share = batch_refs(W, ids, ps, refs);
   BatchSolver<T, C, P, PC> S(h->arena, h->stream, h->opt);
+  if (what >= 3) {  // the transposed (adjoint) operator / preconditioner of the tensorial path: an adjoint batch
+    if (!W.setups[0].tensorial || level != 0 || (what == 3 && mode != 0 && mode != 1)) {
+      h->err = "b200ms_debug_batch: what 3 / 4 (transposed operator / preconditioner) take tensorial problems, level 0 and mode 0 or 1";
+      return B200MS_ERR_ARG;
+    }
+    S.adjoint_ = true;
+    what -= 3;
+  }
   S.build(ps, share, upload_refs(h, refs, h->stream));
   if (what == 0 && mode >= 16) {  // mode + 16: the multigrid operator (preconditioner precision) also on level 0
     mode -= 16;
@@ -1822,7 +1830,7 @@ int debug_window(b200ms_handle *h, int nprob, const b200ms_problem *prob, const 
 
 int debug_dispatch(b200ms_handle *h, int nprob, const b200ms_problem *prob, int what, int level, int mode, const double *in0,
                    const double *in1, double *out, int *iters, double *relres) {
-  if (!h || nprob < 1 || !prob || !in0 || !out || what < 0 || what > 2) return B200MS_ERR_ARG;
+  if (!h || nprob < 1 || !prob || !in0 || !out || what < 0 || what > 4) return B200MS_ERR_ARG;
   if (cudaSetDevice(h->device) != cudaSuccess) return B200MS_ERR_CUDA;
   h->err.clear();
   try {

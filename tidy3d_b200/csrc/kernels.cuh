@@ -1250,9 +1250,30 @@ struct TensorCell {
     if (i < 0 || j < 0 || i >= nx || j >= ny) return mk(0.0, 0.0);
     return F(11, i, j) * G(i, j) - F(9, i, j) * ld(hx, i, j) - F(10, i, j) * ld(hy, i, j);
   }
+  // ---- the transpose M^T z, z = [z1;z2;z3;z4] read through ex, ey, hx, hy.  Dual intermediates (bilinear, no conjugation):
+  //   Ub = Dxf^T z1 + Dyf^T z2,   Tb = Dxb^T z3 + Dyb^T z4,
+  //   Kb = Ub/ezz + (eyz/ezz) z3 - (exz/ezz) z4,   Gb = Tb/mzz + (myz/mzz) z1 - (mxz/mzz) z2,
+  // and  (M^T z)_Ex = -(ezx/ezz) Ub - Dyf^T Gb + Se_yx z3 - Se_xx z4     (M^T z)_Hx = -(mzx/mzz) Tb - Dyb^T Kb + Sm_yx z1 - Sm_xx z2
+  //      (M^T z)_Ey = -(ezy/ezz) Ub + Dxf^T Gb + Se_yy z3 - Se_xy z4     (M^T z)_Hy = -(mzy/mzz) Tb + Dxb^T Kb + Sm_yy z1 - Sm_xy z2
+  // with (Df^T v)[i] = f0[i] v[i] + f1[i-1] v[i-1] and (Db^T v)[i] = b0[i] v[i] + bm[i+1] v[i+1].
+  __device__ __forceinline__ cplx Ub(int i, int j) const {
+    return CX(0, i) * ld(ex, i, j) + CX(1, i - 1) * ld(ex, i - 1, j) + CY(0, j) * ld(ey, i, j) + CY(1, j - 1) * ld(ey, i, j - 1);
+  }
+  __device__ __forceinline__ cplx Tb(int i, int j) const {
+    return CX(2, i) * ld(hx, i, j) + CX(3, i + 1) * ld(hx, i + 1, j) + CY(2, j) * ld(hy, i, j) + CY(3, j + 1) * ld(hy, i, j + 1);
+  }
+  __device__ __forceinline__ cplx Kb(int i, int j) const {
+    if (i < 0 || j < 0 || i >= nx || j >= ny) return mk(0.0, 0.0);
+    return F(2, i, j) * Ub(i, j) + F(3, i, j) * ld(hx, i, j) - F(4, i, j) * ld(hy, i, j);
+  }
+  __device__ __forceinline__ cplx Gb(int i, int j) const {
+    if (i < 0 || j < 0 || i >= nx || j >= ny) return mk(0.0, 0.0);
+    return F(11, i, j) * Tb(i, j) + F(12, i, j) * ld(ex, i, j) - F(13, i, j) * ld(ey, i, j);
+  }
 };
 
-template <typename C>
+// y = (mat - sigma) w  or  rhs - (mat - sigma) w;  TR: the same with mat^T = msign (-i) M^T (left eigenvectors)
+template <typename C, bool TR>
 __global__ void __launch_bounds__(256) tensor_apply_kernel(TensorArgs<C> a) {
   const int nx = a.nx, ny = a.ny;
   const size_t N = (size_t)nx * ny;
@@ -1262,13 +1283,24 @@ __global__ void __launch_bounds__(256) tensor_apply_kernel(TensorArgs<C> a) {
   TensorCell<C> t{wb, wb + N, wb + 2 * N, wb + 3 * N, a.ft + a.ft_bstride * b, a.cx + (size_t)b * 4 * nx, a.cy + (size_t)b * 4 * ny, nx, ny, N};
   const size_t g = (size_t)i * ny + j;
   const cplx ex = ldg(t.ex + g), ey = ldg(t.ey + g), hx = ldg(t.hx + g), hy = ldg(t.hy + g);
-  const cplx u00 = t.U(i, j), u10 = t.U(i + 1, j), u01 = t.U(i, j + 1);
-  const cplx t00 = t.Tt(i, j), tm0 = t.Tt(i - 1, j), t0m = t.Tt(i, j - 1);
-  const cplx kk = t.K(i, j), gg = t.G(i, j);
-  cplx r1 = t.CX(0, i) * u00 + t.CX(1, i) * u10 + t.F(12, i, j) * gg + t.F(16, i, j) * hx + t.F(17, i, j) * hy;
-  cplx r2 = t.CY(0, j) * u00 + t.CY(1, j) * u01 - t.F(13, i, j) * gg - t.F(14, i, j) * hx - t.F(15, i, j) * hy;
-  cplx r3 = t.CX(2, i) * t00 + t.CX(3, i) * tm0 + t.F(3, i, j) * kk + t.F(7, i, j) * ex + t.F(8, i, j) * ey;
-  cplx r4 = t.CY(2, j) * t00 + t.CY(3, j) * t0m - t.F(4, i, j) * kk - t.F(5, i, j) * ex - t.F(6, i, j) * ey;
+  cplx r1, r2, r3, r4;
+  if constexpr (TR) {
+    const cplx ub = t.Ub(i, j), tb = t.Tb(i, j);
+    const cplx g00 = t.Gb(i, j), gm0 = t.Gb(i - 1, j), g0m = t.Gb(i, j - 1);
+    const cplx k00 = t.Kb(i, j), k10 = t.Kb(i + 1, j), k01 = t.Kb(i, j + 1);
+    r1 = -(t.F(0, i, j) * ub) - (t.CY(0, j) * g00 + t.CY(1, j - 1) * g0m) + t.F(7, i, j) * hx - t.F(5, i, j) * hy;
+    r2 = -(t.F(1, i, j) * ub) + (t.CX(0, i) * g00 + t.CX(1, i - 1) * gm0) + t.F(8, i, j) * hx - t.F(6, i, j) * hy;
+    r3 = -(t.F(9, i, j) * tb) - (t.CY(2, j) * k00 + t.CY(3, j + 1) * k01) + t.F(16, i, j) * ex - t.F(14, i, j) * ey;
+    r4 = -(t.F(10, i, j) * tb) + (t.CX(2, i) * k00 + t.CX(3, i + 1) * k10) + t.F(17, i, j) * ex - t.F(15, i, j) * ey;
+  } else {
+    const cplx u00 = t.U(i, j), u10 = t.U(i + 1, j), u01 = t.U(i, j + 1);
+    const cplx t00 = t.Tt(i, j), tm0 = t.Tt(i - 1, j), t0m = t.Tt(i, j - 1);
+    const cplx kk = t.K(i, j), gg = t.G(i, j);
+    r1 = t.CX(0, i) * u00 + t.CX(1, i) * u10 + t.F(12, i, j) * gg + t.F(16, i, j) * hx + t.F(17, i, j) * hy;
+    r2 = t.CY(0, j) * u00 + t.CY(1, j) * u01 - t.F(13, i, j) * gg - t.F(14, i, j) * hx - t.F(15, i, j) * hy;
+    r3 = t.CX(2, i) * t00 + t.CX(3, i) * tm0 + t.F(3, i, j) * kk + t.F(7, i, j) * ex + t.F(8, i, j) * ey;
+    r4 = t.CY(2, j) * t00 + t.CY(3, j) * t0m - t.F(4, i, j) * kk - t.F(5, i, j) * ex - t.F(6, i, j) * ey;
+  }
   const cplx mi = mk(0.0, -a.msign);  // msign * (-i)
   const cplx sg = ldg(a.sigma + b);
   cplx o1 = mi * r1 - sg * ex, o2 = mi * r2 - sg * ey, o3 = mi * r3 - sg * hx, o4 = mi * r4 - sg * hy;
@@ -1335,6 +1367,32 @@ __global__ void __launch_bounds__(256) lin2_kernel(size_t len, const cplx *ca, c
     cplx v = a * ldg(x + x_bstride * b + e);
     if (y) v = v + bb * ldg(y + y_bstride * b + e);
     out[out_bstride * b + e] = v;
+  }
+}
+
+// Local pairing of the diagonal-tensor part of the first-order operator, K mat_d = -mat_d^T K (oracle/tensor_derivatives.py):
+//   K [Ex;Ey;Hx;Hy] = [gx Hy; -gy Hx; gy Ey; -gx Ex],  gx = lf_x lb_y (Ex sites),  gy = lb_x lf_y (Ey sites),
+// with the complex-stretched primal / dual lengths g[b][0][i] = lf[i], g[b][1][i] = lb[i] (halved at a PMC wall).
+// inverse = 0: y = scale K x;  1: y = scale K^-1 x.  Each thread reads its site's four values before writing: y may alias x.
+__global__ void __launch_bounds__(256) tensor_pair_kernel(int inverse, double scale, int nx, int ny, const cplx *gxs, const cplx *gys,
+                                                          const cplx *x, cplx *y) {
+  const size_t N = (size_t)nx * ny;
+  const int j = blockIdx.x * 64 + threadIdx.x, i = blockIdx.y * 4 + threadIdx.y, b = blockIdx.z;
+  if (i >= nx || j >= ny) return;
+  const cplx *gx = gxs + (size_t)b * 2 * nx, *gy = gys + (size_t)b * 2 * ny;
+  const size_t g = (size_t)i * ny + j, o = (size_t)b * 4 * N + g;
+  cplx ge = ldg(gx + i) * ldg(gy + ny + j), gh = ldg(gx + nx + i) * ldg(gy + j);
+  if (inverse) {
+    ge = recip(ge);
+    gh = recip(gh);
+  }
+  ge = scale * ge;
+  gh = scale * gh;
+  const cplx x1 = x[o], x2 = x[o + N], x3 = x[o + 2 * N], x4 = x[o + 3 * N];
+  if (inverse) {
+    y[o] = -(ge * x4); y[o + N] = gh * x3; y[o + 2 * N] = -(gh * x2); y[o + 3 * N] = ge * x1;
+  } else {
+    y[o] = ge * x4; y[o + N] = -(gh * x3); y[o + 2 * N] = gh * x2; y[o + 3 * N] = -(ge * x1);
   }
 }
 

@@ -132,6 +132,9 @@ class BatchSolver {
   bool tensor_ = false;
   bool masked_ = false;      // incidence-matrix formulation: unknowns marked by exx == 0 / eyy == 0 are held at zero
   bool single_out_ = false;  // fields are delivered as complex64 (mode_spec.precision == "single")
+  // tensorial, set before build(): the Krylov-side operator and the preconditioner act with mat^T (left eigenvectors); only
+  // such a batch allocates and uploads the pairing metric and the +sigma scalars of precondition_tensor_T
+  bool adjoint_ = false;
   double msign_ = 1.0;
   bool has_mu = false, shared_fields = false;
   std::vector<Level> lv;
@@ -234,7 +237,11 @@ class BatchSolver {
     if (tensor_) {
       sz.add<C>(fB * 18 * N);
       sz.add<T>(vsE * 6);
-      sz.add<cplx>((size_t)B * 8);
+      sz.add<cplx>((size_t)B * (adjoint_ ? 16 : 8));
+      if (adjoint_) {
+        sz.add<cplx>((size_t)B * 2 * nx);
+        sz.add<cplx>((size_t)B * 2 * ny);
+      }
     }
     coarse_krylov_ = kh_limit > 0.0;
     kc_ = std::max(2, std::min(opt_.mg_coarse_iters, std::max(m, restart) - 1));
@@ -394,21 +401,47 @@ class BatchSolver {
     if (tensor_) {
       ft_ = arena_.get<C>(fB * 18 * N);
       for (int q = 0; q < 6; ++q) tb_[q] = arena_.get<T>(vsE);
-      tcoef_ = arena_.get<cplx>((size_t)B * 8);
+      tcoef_ = arena_.get<cplx>((size_t)B * (adjoint_ ? 16 : 8));
       {
         dim3 grd((unsigned)std::min<size_t>((N + 255) / 256, 2048), (unsigned)fB);
         tensor_fields_kernel<C><<<grd, 256, 0, st_>>>(d_refs, ft_, (size_t)18 * N);
         stats.launches++;
         CUDA_CHECK(cudaGetLastError());
       }
-      // per-problem scalars of the preconditioner: [0] -sigma_t, [1] i*msign, [2] 1/s, [3] -1/s, [4] 1  (s = -sigma_t^2)
-      std::vector<cplx> hc((size_t)B * 8);
+      // per-problem scalars of the preconditioner: [0] -sigma_t, [1] i*msign, [2] 1/s, [3] -1/s, [4] 1  (s = -sigma_t^2);
+      // adjoint batch: at 8 B the same set for the shift +sigma_t, which the transposed preconditioner inverts through (s does
+      // not change)
+      std::vector<cplx> hc((size_t)B * (adjoint_ ? 16 : 8));
       for (int b = 0; b < B; ++b) {
         const cd st = ps[b]->sigma_t, sd = -st * st;
         const cd v[5] = {-st, cd(0, msign_), 1.0 / sd, -1.0 / sd, cd(1, 0)};
-        for (int q = 0; q < 5; ++q) hc[(size_t)q * B + b] = mk(v[q].real(), v[q].imag());
+        for (int q = 0; q < 5; ++q) {
+          hc[(size_t)q * B + b] = mk(v[q].real(), v[q].imag());
+          if (adjoint_) hc[(size_t)(8 + q) * B + b] = q == 0 ? mk(st.real(), st.imag()) : hc[(size_t)q * B + b];
+        }
       }
       CUDA_CHECK(cudaMemcpyAsync(tcoef_, hc.data(), hc.size() * sizeof(cplx), cudaMemcpyHostToDevice, st_));
+      if (adjoint_) {
+        // metric of the pairing K (tensor_pair_kernel): complex-stretched primal / dual lengths, the first dual cell halved at a
+        // PMC wall
+        tgx_ = arena_.get<cplx>((size_t)B * 2 * nx);
+        tgy_ = arena_.get<cplx>((size_t)B * 2 * ny);
+        std::vector<cplx> hg[2];
+        for (int a = 0; a < 2; ++a) {
+          const int n = a == 0 ? nx : ny;
+          hg[a].resize((size_t)B * 2 * n);
+          for (int b = 0; b < B; ++b) {
+            const Axis &A = ps[b]->ax[a];
+            for (int i = 0; i < n; ++i) {
+              const cd lb = (i == 0 && A.pmc) ? 0.5 * A.lb[i] : A.lb[i];
+              hg[a][(size_t)b * 2 * n + i] = mk(A.lf[i].real(), A.lf[i].imag());
+              hg[a][(size_t)b * 2 * n + n + i] = mk(lb.real(), lb.imag());
+            }
+          }
+        }
+        CUDA_CHECK(cudaMemcpyAsync(tgx_, hg[0].data(), hg[0].size() * sizeof(cplx), cudaMemcpyHostToDevice, st_));
+        CUDA_CHECK(cudaMemcpyAsync(tgy_, hg[1].data(), hg[1].size() * sizeof(cplx), cudaMemcpyHostToDevice, st_));
+      }
       CUDA_CHECK(cudaStreamSynchronize(st_));
     }
     if (coarse_krylov_) {
@@ -787,7 +820,8 @@ class BatchSolver {
         a.ft = ft_; a.ft_bstride = shared_fields ? 0 : 18 * N; a.cx = lv[0].cx_true; a.cy = lv[0].cy_true;
         a.sigma = sigma_; a.msign = msign_;
         dim3 blk(64, 4), grd((ny + 63) / 64, (nx + 3) / 4, B);
-        tensor_apply_kernel<C><<<grd, blk, 0, st_>>>(a);
+        if (adjoint_) tensor_apply_kernel<C, true><<<grd, blk, 0, st_>>>(a);
+        else tensor_apply_kernel<C, false><<<grd, blk, 0, st_>>>(a);
         stats.launches++;
         return;
       }
@@ -813,9 +847,10 @@ class BatchSolver {
   // Tensorial preconditioner: z ~ (mat_d - sigma)^-1 v with mat_d = msign (-i) [[0,P],[Q,0]] the diagonal-tensor part:
   //   (mat_d - sigma)^-1 = -(mat_d + sigma) blockdiag((PQ - s)^-1, (QP - s)^-1),  s = -sigma^2,
   //   (PQ - s)^-1 ~ B_E = the multigrid V-cycle of the diagonal path,  (QP - s)^-1 = -(1/s) (I - Q B_E P).
-  // The off-diagonal tensor terms are left to the outer FGMRES.
-  void precondition_tensor(const T *v, T *z) {
-    const cplx *c_negsig = tcoef_, *c_ims = tcoef_ + B, *c_is = tcoef_ + 2 * B, *c_mis = tcoef_ + 3 * B, *c_one = tcoef_ + 4 * B;
+  // The off-diagonal tensor terms are left to the outer FGMRES.  coef: the scalar set (tcoef_ for -sigma_t, tcoef_ + 8 B for
+  // +sigma_t).  Every read of v precedes the first write of z, so z may alias v.
+  void precondition_tensor(const T *v, T *z, const cplx *coef) {
+    const cplx *c_negsig = coef, *c_ims = coef + B, *c_is = coef + 2 * B, *c_mis = coef + 3 * B, *c_one = coef + 4 * B;
     const T *ve = v, *vh = v + lenE;
     T *ye = tb_[0], *t1 = tb_[1], *g = tb_[2], *t2 = tb_[3], *yh = tb_[4], *t3 = tb_[5];
     precondition_E(ve, len, ye, lenE);          // y_e = B_E v_e
@@ -828,6 +863,20 @@ class BatchSolver {
     apply_pq(1, ye, lenE, t3, lenE);            // Q y_e
     lin2(c_negsig, yh, lenE, c_ims, t3, lenE, z + lenE, len);   // z_h = -sigma y_h + i msign Q y_e
     (void)c_one;
+  }
+  // Transposed tensorial preconditioner: z ~ (mat_d^T - sigma)^-1 v.  The pairing K mat_d = -mat_d^T K (tensor_pair_kernel) gives
+  //   (mat_d^T - sigma)^-1 = -K (mat_d + sigma)^-1 K^-1,
+  // and (mat_d + sigma)^-1 is precondition_tensor with the shift negated: s = -sigma^2 and so the multigrid are unchanged.
+  void precondition_tensor_T(const T *v, T *z) {
+    if constexpr (std::is_same<T, cplx>::value) {
+      dim3 blk(64, 4), grd((ny + 63) / 64, (nx + 3) / 4, B);
+      tensor_pair_kernel<<<grd, blk, 0, st_>>>(1, 1.0, nx, ny, tgx_, tgy_, v, z);
+      CUDA_CHECK(cudaGetLastError());
+      precondition_tensor(z, z, tcoef_ + 8 * B);
+      tensor_pair_kernel<<<grd, blk, 0, st_>>>(0, -1.0, nx, ny, tgx_, tgy_, z, z);
+      CUDA_CHECK(cudaGetLastError());
+      stats.launches += 2;
+    }
   }
   // the multigrid operator on level l (preconditioner precision, phase-limited PML)
   void apply(int l, int mode, const P *x, const P *rhs, P *y) {
@@ -855,8 +904,10 @@ class BatchSolver {
   // residual), converting on the way in and out when the multigrid runs in fp32.  Two cycles per application roughly
   // halve the FGMRES iteration count, which pays because the Gram-Schmidt cost grows quadratically with it.
   void precondition(const T *v, T *z) {
-    if (tensor_) {
-      precondition_tensor(v, z);
+    if (tensor_ && adjoint_) {
+      precondition_tensor_T(v, z);
+    } else if (tensor_) {
+      precondition_tensor(v, z, tcoef_);
     } else {
       precondition_E(v, len, z, len);
       mask_E(z, len);
@@ -2318,7 +2369,7 @@ class BatchSolver {
   P *sigma_p_ = nullptr, *pre_a_ = nullptr, *pre_b_ = nullptr;
   C *ft_ = nullptr;
   T *tb_[6] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
-  cplx *tcoef_ = nullptr;
+  cplx *tcoef_ = nullptr, *tgx_ = nullptr, *tgy_ = nullptr;
   std::vector<cd> sig_mg_host_;
   bool dinv_ready_ = false;
   int sms_ = 0;  // streaming multiprocessors of the device
