@@ -280,7 +280,9 @@ typedef struct {
   int transfer_vec;      /* multigrid transfers: bit 0 = the prolongation reads / writes its four fine values as one 128-bit access (fp32 vectors,
                             nyf % 4 == 0); bit 1 = the restriction reads packed lists of up to four entries; bit 2 (with bit 1) = on levels the
                             TMA pair kernel covers in one strip, the residual is restricted inside the residual kernel and never stored (same
-                            results bit for bit).  Default 7; 3 gives the separate residual and restriction kernels */
+                            results bit for bit); bit 3 = on those levels, with mg_nu == 2 and mg_nu_growth == 0, the prolongation and both
+                            post-smoothing sweeps run as one pass (same results bit for bit).  Default 15; 7 gives the separate prolongation
+                            and sweeps, 3 also the separate residual and restriction kernels */
   int tensor_mg_cycles;  /* tensorial path: V-cycles (defect correction on the multigrid operator) per application of the E-block inverse inside
                             the block preconditioner; 0 = mg_cycles.  Default 3 (see csrc/solver.cuh mg_cycles_ and tools/proto_tensor.py) */
 } b200ms_options;
@@ -322,7 +324,9 @@ int b200ms_solve_batch(b200ms_handle *h, int nprob, const b200ms_problem *prob, 
  * of the operator of `prob` and return the mean kernel time (CUDA events on the library stream).
  * mode 0: y = (A - sigma) x, the fp64 operator apply of the Krylov iteration; mode 1: the production smoother sweep
  * (stored-diagonal Jacobi in the multigrid precision); mode 2: one fused CGS2 Gram-Schmidt step of the inner solver against
- * four basis vectors in the multigrid precision (gs_dots, gs_update_dots, gs_update_norm, gs_scale: 19 vector passes).  x (2*nx*ny complex128 (re,im)) may be NULL (random); y may be
+ * four basis vectors in the multigrid precision (gs_dots, gs_update_dots, gs_update_norm, gs_scale: 19 vector passes); mode 3: the
+ * post-smoothing of level 0 as one pass (prolongation of lv[1].x and two stored-diagonal sweeps, transfer_vec bit 3; an error
+ * where level 0 does not take it); mode 4: the same as the separate prolongation and two sweeps.  x (2*nx*ny complex128 (re,im)) may be NULL (random); y may be
  * NULL.  bytes_per_apply returns the algorithmic bytes of one launch (SURVEY 8(d)): N*(4*s_v + nf*s_c) per problem for
  * the apply, N*(8*s_v + nf*s_c) for the sweep. */
 int b200ms_bench_stencil(b200ms_handle *h, const b200ms_problem *prob, int nbatch, int mode, int nrep,
@@ -376,7 +380,8 @@ int b200ms_debug_post_tables_bounded(const double *coords, int n, int sym, doubl
  *                  Vectors have 2 nx_l ny_l elements per problem.
  *   what 1: one preconditioner application out = M^-1 in (the multigrid V-cycle; tensorial: the block preconditioner);
  *           *iters (when not NULL) gets a bit mask of the levels whose residual was restricted inside the residual kernel
- *           (transfer_vec bit 2).
+ *           (transfer_vec bit 2) in bits 0-15, and of the levels whose prolongation and post-smoothing ran as one pass
+ *           (transfer_vec bit 3) in bits 16 + level.
  *   what 2: out = (A - sigma)^-1 in by the inner solver of the eigen-iteration, to the handle's inner_tol; *iters gets its
  *           Arnoldi steps, relres[nprob] the final relative residual of every problem.
  *   Tensorial problems only (else B200MS_ERR_ARG), level 0; these two modes change no struct, so they carry no version of their

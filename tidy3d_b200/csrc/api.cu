@@ -117,7 +117,7 @@ extern "C" void b200ms_default_options(b200ms_options *o) {
   o->outer_dgks = 1;
   o->stencil_pair = 4;
   o->stencil_pair_rows = 0;
-  o->transfer_vec = 7;
+  o->transfer_vec = 15;
   o->tensor_mg_cycles = 3;
 }
 
@@ -1504,8 +1504,22 @@ static void bench_group(b200ms_handle *h, const Window &W, int nbatch, int mode,
     for (int q = 0; q < 5; ++q)
       for (int b = 0; b < nbatch; ++b)
         CUDA_CHECK(cudaMemcpyAsync(gsV + (size_t)q * S.vstride + (size_t)b * len, hp.data(), len * sizeof(P), cudaMemcpyHostToDevice, h->stream));
+  // modes 3 / 4: the post-smoothing of level 0 from the coarse correction lv[1].x -- the fused pass (3), or the prolongation
+  // and two stored-diagonal sweeps as separate kernels (4)
+  if (mode == 3 && !S.fused_post_levels()) throw std::runtime_error("b200ms_bench_stencil mode 3: level 0 does not take the fused post-smoothing pass");
+  if ((mode == 3 || mode == 4) && S.lv.size() < 2) throw std::runtime_error("b200ms_bench_stencil mode 3 / 4: the hierarchy has one level");
+  if (mode == 3 || mode == 4) {
+    const size_t nc = (size_t)nbatch * 2 * S.lv[1].N;
+    fill_kernel<P><<<(unsigned)std::min<size_t>((nc + 255) / 256, 8192), 256, 0, h->stream>>>(nc, from_real<P>(0.25), S.lv[1].x);
+  }
   auto run = [&]() {
-    if (mode == 2) S.template gs_cgs2<P>(gsV, S.vstride, len, 4, gsW, gsW, nullptr, reinterpret_cast<P *>(S.hessenberg()), (size_t)S.restart * (S.restart + 4));
+    if (mode == 3) {
+      S.prolong_jacobi2(0, px, prhs, py);
+    } else if (mode == 4) {
+      S.prolong_add(0, px);
+      S.apply(0, MODE_JACOBI, px, prhs, py);
+      S.apply(0, MODE_JACOBI, py, prhs, px);
+    } else if (mode == 2) S.template gs_cgs2<P>(gsV, S.vstride, len, 4, gsW, gsW, nullptr, reinterpret_cast<P *>(S.hessenberg()), (size_t)S.restart * (S.restart + 4));
     else if (mode == 1) S.apply(0, MODE_JACOBI, px, prhs, py);
     else S.apply_true(MODE_APPLY, dx, drhs, dy);
   };
@@ -1538,6 +1552,10 @@ static void bench_group(b200ms_handle *h, const Window &W, int nbatch, int mode,
   const double ncell = (double)S.N * nbatch;
   if (bytes_out && mode == 2)  // dots: 4+1 vectors; update+dots: 4 + r/w w; update+norm: 4 + r/w w; scale: r + w
     *bytes_out = (double)len * nbatch * sizeof(P) * 19.0;
+  else if (bytes_out && (mode == 3 || mode == 4))  // x, rhs, omega/diag, output (8) + coefficient fields per sweep, + the coarse correction;
+                                                   // separately: read + write x for the prolongation and all of it twice
+    *bytes_out = ncell * (mode == 3 ? 8.0 * sizeof(P) + (double)S.nf * sizeof(PC) : 20.0 * sizeof(P) + 2.0 * S.nf * sizeof(PC)) +
+                 (double)nbatch * 2 * S.lv[1].N * sizeof(P);
   else if (bytes_out)
     *bytes_out = mode == 1 ? ncell * (8.0 * sizeof(P) + (double)S.nf * sizeof(PC)) : ncell * (4.0 * sizeof(T) + (double)S.nf * sizeof(C));
   if (y) {
@@ -1791,7 +1809,7 @@ int debug_run(b200ms_handle *h, const Window &W, int what, int level, int mode, 
     S.apply_true(mode, d0, d1, d2);
   } else if (what == 1) {
     S.precondition(d0, d2);
-    if (iters) *iters = S.resid_restrict_levels();
+    if (iters) *iters = S.resid_restrict_levels() | S.fused_post_levels() << 16;
   } else {
     int it = 0;
     std::vector<double> rr;

@@ -153,7 +153,8 @@ __global__ void __launch_bounds__(256) convert_kernel(size_t total, const S *src
 // _D: stored omega/diag.  _D0: two sweeps from a zero guess in one pass, x' = x0 + dinv (rhs - (A-sigma) x0) with x0 = dinv rhs formed
 // while the rows are loaded (replaces the separate dinv*rhs product kernel and the x read of the first sweep)
 // _RESTRICT: the residual is restricted to the next coarser level inside the march (csrc/march2_tma.cuh) and never stored
-enum { MODE_APPLY = 0, MODE_RESID = 1, MODE_JACOBI = 2, MODE_JACOBI_D = 3, MODE_JACOBI_D0 = 4, MODE_RESID_RESTRICT = 5 };
+// _PROLONG_JACOBI2: the prolongation x + P e_c followed by two stored-diagonal sweeps in one march (csrc/march2_tma.cuh)
+enum { MODE_APPLY = 0, MODE_RESID = 1, MODE_JACOBI = 2, MODE_JACOBI_D = 3, MODE_JACOBI_D0 = 4, MODE_RESID_RESTRICT = 5, MODE_PROLONG_JACOBI2 = 6 };
 
 struct TransferArgs;
 
@@ -170,8 +171,8 @@ struct StencilArgs {
   const T *sigma;    // [B]
   double omega;      // Jacobi damping
   const T *dinv;     // [B][2][N] omega / diag(A - sigma) (MODE_JACOBI_D)
-  const TransferArgs *tr;  // device copy of the transfer lists to the next coarser level (MODE_RESID_RESTRICT)
-  T *coarse;               // [B][2][Nc] restricted residual (MODE_RESID_RESTRICT)
+  const TransferArgs *tr;  // device copy of the transfer lists to the next coarser level (MODE_RESID_RESTRICT, MODE_PROLONG_JACOBI2)
+  T *coarse;               // [B][2][Nc] restricted residual (MODE_RESID_RESTRICT) / coarse correction read (MODE_PROLONG_JACOBI2)
 };
 
 template <typename T> struct Tile;

@@ -55,6 +55,14 @@ __device__ __forceinline__ void bulk_g2s(void *smem_dst, const void *gmem_src, u
                "r"(bytes), "r"(smem_u32(bar))
                : "memory");
 }
+// one 4-byte asynchronous copy (LDGSTS), and an arrival on `bar` once this thread's earlier ones have landed (the barrier's
+// expected arrival count includes it)
+__device__ __forceinline__ void cp_async4(void *smem_dst, const void *gmem_src) {
+  asm volatile("cp.async.ca.shared.global [%0], [%1], 4;\n" ::"r"(smem_u32(smem_dst)), "l"(gmem_src) : "memory");
+}
+__device__ __forceinline__ void cp_async_arrive(unsigned long long *bar) {
+  asm volatile("cp.async.mbarrier.arrive.noinc.shared::cta.b64 [%0];\n" ::"r"(smem_u32(bar)) : "memory");
+}
 
 template <int MODE>
 struct M2TmaArrays {
@@ -288,6 +296,271 @@ __global__ void __launch_bounds__(kM2MaxW, 2) stencil_march2_tma_kernel(StencilA
           ++nI;
         }
       }
+    }
+  }
+}
+
+// MODE_PROLONG_JACOBI2: the post-smoothing half of a V(2,2) level in one march -- the prolongation x = x_old + P e_c and two
+// stored-diagonal sweeps -- in place of prolong_add4_kernel (prolong_add_kernel) and two MODE_JACOBI_D passes.  Row step j
+// (row k = k0 + j) runs three stages:
+//   0. raw row k+2: x_old out of the ring plus P e_c, prolong_add4_kernel's sum with its contractions; the four coarse rows
+//      it reads (x-edge lists for component 0, x-node lists for component 1) are staged into the same ring stage by 4-byte
+//      cp.async that arrive on the stage's barrier (coarse rows need not be 16-byte aligned);
+//   1. sweep 1 (the march of stencil_march2_tma_kernel<MODE_JACOBI_D>) with output row k, kept in the thread's registers;
+//   2. sweep 2, the same march one pipeline later: row k of sweep 1 is its newest row, its output row k - 2 goes to a.y.
+// Sweep 2 needs exx / eyy / 1/ezz of row k and rhs / omega-over-diagonal of row k - 2: the ring stage of step j - 2 holds
+// both, so the ring has kPjRing = 4 stages (steps j - 2 .. j and one in flight) and a stage is refilled once sweep 2 has
+// read it.  A CTA owns the output rows [i0, i0 + rows); it runs sweep 1 on [i0 - 1, i0 + rows] and the prolongation on
+// [i0 - 2, i0 + rows + 1], rows its neighbours also compute.  One strip per row; rows % 6 == 0 and rows + 6 <= kM2MaxSteps
+// (host: fused_post_plan in csrc/solver.cuh).  a.y never aliases a.x.
+// The row-step arithmetic carries explicit roundings (pj_u, pj_t, pj_sweep): the contractions the compiler gives
+// stencil_march2_tma_kernel<MODE_JACOBI_D> (its PTX, plus the multiply-subtract pairs ptxas fuses) depend on the code around
+// the expressions, so the same source in this kernel would round differently.  tests/test_gpu_fused_post_smoothing.py holds
+// the two to the same bits.
+constexpr int kPjRing = 4;
+constexpr int kPjArr = 9;  // x_old (2), exx, eyy, 1/ezz of the raw row; rhs (2) and omega/diag (2) of sweep 1's output row
+__host__ __device__ inline size_t pj_stage_floats(int W, int nyc) { return (size_t)kPjArr * 2 * W + 4 * (size_t)((nyc + 3) & ~3); }
+inline size_t pj_smem(int W, int nyc) { return kPjRing * pj_stage_floats(W, nyc) * sizeof(float); }
+
+// x + P e_c at one fine value out of the coarse rows c0 (I0) and c1 (I1)
+__device__ __forceinline__ float pj_prolong(float x, float wx0, float wx1, const float *c0, const float *c1, int J0, int J1, float wy0,
+                                            float wy1) {
+  return __fadd_rn(x, __fmaf_rn(wx0, __fmaf_rn(wy0, c0[J0], __fmul_rn(wy1, c0[J1])), __fmul_rn(wx1, __fmaf_rn(wy0, c1[J0], __fmul_rn(wy1, c1[J1])))));
+}
+
+// u = -(1/ezz (b0 a1 + bm a0 + yb0 b1 + ybm bl)) and t = f0 v21 + f1 v22 - yf0 v11 - yf1 v11' of the march
+__device__ __forceinline__ float pj_u(float ie, float b0, float a1, float bm, float a0, float yb0, float b1, float ybm, float bl) {
+  return -__fmul_rn(ie, __fmaf_rn(ybm, bl, __fmaf_rn(yb0, b1, __fmaf_rn(b0, a1, __fmul_rn(bm, a0)))));
+}
+__device__ __forceinline__ float pj_t(float f0, float v21, float f1, float v22, float yf0, float v11, float yf1, float v11r) {
+  return __fmaf_rn(-yf1, v11r, __fmaf_rn(-yf0, v11, __fmaf_rn(f0, v21, __fmul_rn(f1, v22))));
+}
+// the stored-diagonal sweep's output pair of row k: x + (omega/diag) (rhs - (A - sigma) x), both components
+__device__ __forceinline__ void pj_sweep(const RowCoef<float> &xc, float2 yf0, float2 yf1, float2 yb0, float2 ybm, float sg, float2 u0,
+                                         float2 u1, float ur, float2 t0, float2 tm, float tl, float2 a0, float2 b0, float2 v10,
+                                         float2 v20, float2 cr1, float2 cr2, float2 cd1, float2 cd2, float2 &w1, float2 &w2) {
+  const float p1x = __fmaf_rn(xc.f0, u0.x, __fmul_rn(xc.f1, u1.x)), p1y = __fmaf_rn(xc.f0, u0.y, __fmul_rn(xc.f1, u1.y));
+  const float p2x = __fmaf_rn(yf1.x, u0.y, __fmul_rn(yf0.x, u0.x)), p2y = __fmaf_rn(yf0.y, u0.y, __fmul_rn(yf1.y, ur));
+  const float c1x = __fsub_rn(__fmaf_rn(yb0.x, t0.x, __fmul_rn(ybm.x, tl)), a0.x), c1y = __fsub_rn(__fmaf_rn(yb0.y, t0.y, __fmul_rn(ybm.y, t0.x)), a0.y);
+  const float c2x = __fadd_rn(__fmaf_rn(xc.bm, tm.x, __fmul_rn(xc.b0, t0.x)), b0.x), c2y = __fadd_rn(__fmaf_rn(xc.bm, tm.y, __fmul_rn(xc.b0, t0.y)), b0.y);
+  const float o1x = __fmaf_rn(-sg, v10.x, __fadd_rn(p1x, c1x)), o1y = __fmaf_rn(-sg, v10.y, __fadd_rn(p1y, c1y));
+  const float o2x = __fmaf_rn(-sg, v20.x, __fsub_rn(p2x, c2x)), o2y = __fmaf_rn(-sg, v20.y, __fsub_rn(p2y, c2y));
+  w1 = make_float2(__fmaf_rn(cd1.x, __fsub_rn(cr1.x, o1x), v10.x), __fmaf_rn(cd1.y, __fsub_rn(cr1.y, o1y), v10.y));
+  w2 = make_float2(__fmaf_rn(cd2.x, __fsub_rn(cr2.x, o2x), v20.x), __fmaf_rn(cd2.y, __fsub_rn(cr2.y, o2y), v20.y));
+}
+
+__global__ void __launch_bounds__(kM2MaxW, 2) stencil_prolong_jacobi2_kernel(StencilArgs<float, float> a, int rows) {
+  using T = float;
+  using V = float2;
+  __shared__ T sB[2][2][kM2MaxW + 2], sV[2][2][kM2MaxW + 2], sU[2][2][kM2MaxW + 2], sTt[2][2][kM2MaxW + 2];  // [sweep][buffer]
+  __shared__ RowCoef<T> sX[kM2MaxSteps + 3];  // coefficients of rows k0 - 2 ..
+  __shared__ int4 sPi[kM2MaxSteps];           // coarse rows of raw row k0 + 2 + j: x-edge I0, I1, x-node I0, I1
+  __shared__ float4 sPw[kM2MaxSteps];         // and their weights
+  __shared__ __align__(8) unsigned long long sBar[kPjRing];
+  extern __shared__ __align__(128) unsigned char m2_ring_raw[];  // [kPjRing][kPjArr][W] float2, then [4][nyc rounded to 4] floats
+  T *ring = reinterpret_cast<T *>(m2_ring_raw);
+
+  const TransferArgs &tr = *a.tr;
+  const int nx = a.nx, ny = a.ny, nyc = tr.nyc;
+  const int nycp = (nyc + 3) & ~3;
+  const int W = blockDim.x;
+  const unsigned N = (unsigned)nx * (unsigned)ny;
+  const size_t Nc = (size_t)tr.nxc * nyc;
+  const int b = blockIdx.z;
+  const int c = threadIdx.x;
+  const int npairs = ny >> 1;
+  const int gj = 2 * c;
+  const bool colv = c < npairs;
+  const int i0 = blockIdx.y * rows;
+  const int iend = (i0 + rows < nx) ? i0 + rows : nx;
+  const int k0 = i0 - 4;
+  const int nsteps = rows + 6;
+  const int raw_lo = max(i0 - 2, 0), raw_hi = min(iend + 1, nx - 1);  // rows the prolongation forms
+  const int s1_lo = max(i0 - 1, 0), s1_hi = min(iend, nx - 1);       // rows sweep 1 outputs
+  const size_t stf = pj_stage_floats(W, nyc);
+  const T *x1 = a.x + (size_t)b * 2 * N, *x2 = x1 + N;
+  const T *fb = a.fields + a.field_bstride * b;
+  const T *exx = fb, *eyy = fb + N, *iez = fb + 2 * (size_t)N;
+  const T *cx = a.cx + (size_t)b * 4 * nx, *cy = a.cy + (size_t)b * 4 * ny;
+  const T *r1 = a.rhs + (size_t)b * 2 * N, *r2 = r1 + N;
+  const T *d1 = a.dinv + (size_t)b * 2 * N, *d2 = d1 + N;
+  const T *cb = a.coarse + (size_t)b * 2 * Nc;  // coarse correction, component 0 (component 1 at + Nc)
+  T *y1 = a.y + (size_t)b * 2 * N, *y2 = y1 + N;
+  const T zT = 0.0f;
+  const V zV = {zT, zT};
+  const unsigned nbytes = (unsigned)npairs * (unsigned)sizeof(V);
+
+  // lanes 0 .. kPjArr-1 of warp 0 each own one array (bulk copies); every thread copies its share of the four coarse rows and
+  // arrives on the stage's barrier (W + 1 arrivals per phase: lane 0's expect_tx and one per thread)
+  const T *my_arr = nullptr;
+  if (c == 0) my_arr = x1; else if (c == 1) my_arr = x2; else if (c == 2) my_arr = exx; else if (c == 3) my_arr = eyy; else if (c == 4) my_arr = iez;
+  else if (c == 5) my_arr = r1; else if (c == 6) my_arr = r2; else if (c == 7) my_arr = d1; else if (c == 8) my_arr = d2;
+  auto issue = [&](int jj) {
+    const int stage = jj & (kPjRing - 1);
+    const int gr = k0 + jj + 2, go = k0 + jj;
+    const bool rawv = gr >= raw_lo && gr <= raw_hi;
+    const bool outv = go >= s1_lo && go <= s1_hi;
+    unsigned long long *bar = &sBar[stage];
+    T *st = ring + stage * stf;
+    if (c == 0) mbar_expect_tx(bar, ((rawv ? 5u : 0u) + (outv ? 4u : 0u)) * nbytes);
+    if (c < kPjArr && (c < 5 ? rawv : outv)) bulk_g2s(st + (size_t)c * 2 * W, my_arr + (size_t)(c < 5 ? gr : go) * ny, nbytes, bar);
+    if (rawv) {
+      const int4 pi = sPi[jj];
+      const int ci[4] = {pi.x, pi.y, pi.z, pi.w};
+      T *cs = st + (size_t)kPjArr * 2 * W;
+#pragma unroll
+      for (int r = 0; r < 4; ++r) {
+        const T *src = cb + (r >> 1) * Nc + (size_t)ci[r] * nyc;
+        for (int e = c; e < nyc; e += W) cp_async4(cs + r * nycp + e, src + e);
+      }
+    }
+    cp_async_arrive(bar);
+  };
+
+  if (c == 0) {
+#pragma unroll
+    for (int s = 0; s < kPjRing; ++s) mbar_init(&sBar[s], W + 1);
+    mbar_fence_init();
+  }
+  for (int r = c; r < nsteps + 3; r += W) {  // coefficients of rows k0 - 2 .. k0 + nsteps
+    const int gi = k0 - 2 + r;
+    RowCoef<T> rc;
+    rc.f0 = rc.f1 = rc.b0 = rc.bm = zT;
+    if (gi >= 0 && gi < nx) { rc.f0 = __ldg(cx + gi); rc.f1 = __ldg(cx + nx + gi); rc.b0 = __ldg(cx + 2 * nx + gi); rc.bm = __ldg(cx + 3 * nx + gi); }
+    sX[r] = rc;
+  }
+  for (int r = c; r < nsteps; r += W) {  // prolongation rows of the raw rows k0 + 2 ..
+    const int gi = k0 + 2 + r;
+    int4 pi = make_int4(0, 0, 0, 0);
+    float4 pw = make_float4(0.f, 0.f, 0.f, 0.f);
+    if (gi >= 0 && gi < nx) {
+      pi = make_int4(__ldg(tr.xe.p_i0 + gi), __ldg(tr.xe.p_i1 + gi), __ldg(tr.xn.p_i0 + gi), __ldg(tr.xn.p_i1 + gi));
+      pw = make_float4(__ldg(tr.xe.p_w0f + gi), __ldg(tr.xe.p_w1f + gi), __ldg(tr.xn.p_w0f + gi), __ldg(tr.xn.p_w1f + gi));
+    }
+    sPi[r] = pi;
+    sPw[r] = pw;
+  }
+  for (int p = 0; p < 2; ++p)
+    for (int s = 0; s < 2; ++s) {
+      sB[p][s][c + 1] = zT; sV[p][s][c + 1] = zT; sU[p][s][c + 1] = zT; sTt[p][s][c + 1] = zT;
+      if (c < 2) {
+        const int e = c == 0 ? 0 : W + 1;
+        sB[p][s][e] = zT; sV[p][s][e] = zT; sU[p][s][e] = zT; sTt[p][s][e] = zT;
+      }
+    }
+  V yf0 = zV, yf1 = zV, yb0 = zV, ybm = zV;
+  // y-lists of the pair's two columns: y-node lists for component 0, y-edge lists for component 1; the coarse column pair
+  // J0 | J1 << 16 per fine column (nyc < 2^16) keeps the two sweeps' pipelines within 128 registers
+  int2 jn = make_int2(0, 0), je = jn;
+  V wn0 = zV, wn1 = zV, we0 = zV, we1 = zV;
+  if (colv) {
+    yf0 = ldg2(cy + gj); yf1 = ldg2(cy + ny + gj); yb0 = ldg2(cy + 2 * ny + gj); ybm = ldg2(cy + 3 * ny + gj);
+    const int2 jn0 = __ldg(reinterpret_cast<const int2 *>(tr.yn.p_i0 + gj)), jn1 = __ldg(reinterpret_cast<const int2 *>(tr.yn.p_i1 + gj));
+    const int2 je0 = __ldg(reinterpret_cast<const int2 *>(tr.ye.p_i0 + gj)), je1 = __ldg(reinterpret_cast<const int2 *>(tr.ye.p_i1 + gj));
+    jn = make_int2(jn0.x | jn1.x << 16, jn0.y | jn1.y << 16);
+    je = make_int2(je0.x | je1.x << 16, je0.y | je1.y << 16);
+    wn0 = ldg2(tr.yn.p_w0f + gj); wn1 = ldg2(tr.yn.p_w1f + gj); we0 = ldg2(tr.ye.p_w0f + gj); we1 = ldg2(tr.ye.p_w1f + gj);
+  }
+  const bool mask_col0 = tr.mask_y && gj == 0 && ny > 1;  // component 0, fine column 0
+  const bool mask_row0 = tr.mask_x && nx > 1;              // component 1, fine row 0
+  const T sg = __ldg(a.sigma + b);
+  __syncthreads();  // barriers initialised, row tables and exchange rows in place
+#pragma unroll
+  for (int s = 0; s < kPjRing; ++s)
+    if (s < nsteps) issue(s);
+
+  // sweep 1 (raw rows: x_old + P e_c) and sweep 2 (raw rows: sweep 1's output), each the register pipeline of the march
+  V a1 = zV, b1 = zV, v11 = zV, v21 = zV, a0 = zV, b0 = zV, v10 = zV, v20 = zV, ie1 = zV;
+  V u0 = zV, t0 = zV, tm = zV;
+  V ha1 = zV, hb1 = zV, hv11 = zV, hv21 = zV, ha0 = zV, hb0 = zV, hv10 = zV, hv20 = zV, hie1 = zV;
+  V hu0 = zV, ht0 = zV, htm = zV;
+  RowCoef<T> xc = sX[2], hxc = sX[0];  // coefficients of the output rows k (sweep 1) and k - 2 (sweep 2)
+
+  // two-fold unroll (the exchange buffer index stays a constant): unrolled six-fold like the kernels above it spills at 128 registers
+  for (int j0 = 0; j0 < nsteps; j0 += 2) {
+#pragma unroll
+    for (int u = 0; u < 2; ++u) {
+      const int j = j0 + u, k = k0 + j;
+      const int s = u & 1, sp = s ^ 1;
+      const int stage = j & (kPjRing - 1);
+      mbar_wait(&sBar[stage], (unsigned)(j / kPjRing) & 1u);
+      const T *stT = ring + stage * stf;
+      const V *st = reinterpret_cast<const V *>(stT);
+      const V *sth = reinterpret_cast<const V *>(ring + ((j - 2) & (kPjRing - 1)) * stf);  // stage of step j - 2
+      // stage 0: raw row k+2 = x_old + P e_c
+      const int gr = k + 2;
+      V v12 = zV, v22 = zV, ex2 = zV, ey2 = zV, ie2 = zV;
+      if (gr >= raw_lo && gr <= raw_hi && colv) {
+        v12 = st[0 * W + c]; v22 = st[1 * W + c]; ex2 = st[2 * W + c]; ey2 = st[3 * W + c]; ie2 = st[4 * W + c];
+        const float4 pw = sPw[j];
+        const T *cs = stT + (size_t)kPjArr * 2 * W;
+        if (!mask_col0) v12.x = pj_prolong(v12.x, pw.x, pw.y, cs, cs + nycp, jn.x & 0xffff, jn.x >> 16, wn0.x, wn1.x);
+        v12.y = pj_prolong(v12.y, pw.x, pw.y, cs, cs + nycp, jn.y & 0xffff, jn.y >> 16, wn0.y, wn1.y);
+        if (!(mask_row0 && gr == 0)) {
+          v22.x = pj_prolong(v22.x, pw.z, pw.w, cs + 2 * nycp, cs + 3 * nycp, je.x & 0xffff, je.x >> 16, we0.x, we1.x);
+          v22.y = pj_prolong(v22.y, pw.z, pw.w, cs + 2 * nycp, cs + 3 * nycp, je.y & 0xffff, je.y >> 16, we0.y, we1.y);
+        }
+      }
+      // stage 1: sweep 1, output row k
+      V a2, b2;
+      a2.x = __fmul_rn(ex2.x, v12.x); a2.y = __fmul_rn(ex2.y, v12.y);
+      b2.x = __fmul_rn(ey2.x, v22.x); b2.y = __fmul_rn(ey2.y, v22.y);
+      sB[0][s][c + 1] = b2.y;
+      sV[0][s][c + 1] = v12.x;
+      const T bl = sB[0][sp][c], v1r = sV[0][sp][c + 2];
+      const RowCoef<T> xn = sX[j + 3];
+      V u1, t1;
+      u1.x = pj_u(ie1.x, xn.b0, a1.x, xn.bm, a0.x, yb0.x, b1.x, ybm.x, bl);
+      u1.y = pj_u(ie1.y, xn.b0, a1.y, xn.bm, a0.y, yb0.y, b1.y, ybm.y, b1.x);
+      t1.x = pj_t(xn.f0, v21.x, xn.f1, v22.x, yf0.x, v11.x, yf1.x, v11.y);
+      t1.y = pj_t(xn.f0, v21.y, xn.f1, v22.y, yf0.y, v11.y, yf1.y, v1r);
+      sU[0][s][c + 1] = u1.x;
+      sTt[0][s][c + 1] = t1.y;
+      const bool s1v = colv && k >= s1_lo && k <= s1_hi;
+      V w1 = zV, w2 = zV;  // sweep 1 at row k (zero outside the rows sweep 2 reads, as its raw rows outside the grid)
+      if (s1v) {
+        const T ur = sU[0][sp][c + 2], tl = sTt[0][sp][c];
+        pj_sweep(xc, yf0, yf1, yb0, ybm, sg, u0, u1, ur, t0, tm, tl, a0, b0, v10, v20, st[5 * W + c], st[6 * W + c], st[7 * W + c],
+                 st[8 * W + c], w1, w2);
+      }
+      // stage 2: sweep 2 with row k of sweep 1 as its newest row, output row k - 2
+      V hex2 = zV, hey2 = zV, hie2 = zV;
+      if (s1v) { hex2 = sth[2 * W + c]; hey2 = sth[3 * W + c]; hie2 = sth[4 * W + c]; }
+      V ha2, hb2;
+      ha2.x = __fmul_rn(hex2.x, w1.x); ha2.y = __fmul_rn(hex2.y, w1.y);
+      hb2.x = __fmul_rn(hey2.x, w2.x); hb2.y = __fmul_rn(hey2.y, w2.y);
+      sB[1][s][c + 1] = hb2.y;
+      sV[1][s][c + 1] = w1.x;
+      const T hbl = sB[1][sp][c], hv1r = sV[1][sp][c + 2];
+      const RowCoef<T> hxn = sX[j + 1];
+      V hu1, ht1;
+      hu1.x = pj_u(hie1.x, hxn.b0, ha1.x, hxn.bm, ha0.x, yb0.x, hb1.x, ybm.x, hbl);
+      hu1.y = pj_u(hie1.y, hxn.b0, ha1.y, hxn.bm, ha0.y, yb0.y, hb1.y, ybm.y, hb1.x);
+      ht1.x = pj_t(hxn.f0, hv21.x, hxn.f1, w2.x, yf0.x, hv11.x, yf1.x, hv11.y);
+      ht1.y = pj_t(hxn.f0, hv21.y, hxn.f1, w2.y, yf0.y, hv11.y, yf1.y, hv1r);
+      sU[1][s][c + 1] = hu1.x;
+      sTt[1][s][c + 1] = ht1.y;
+      const int ko = k - 2;
+      if (colv && ko >= i0 && ko < iend) {
+        const T ur = sU[1][sp][c + 2], tl = sTt[1][sp][c];
+        V z1, z2;
+        pj_sweep(hxc, yf0, yf1, yb0, ybm, sg, hu0, hu1, ur, ht0, htm, tl, ha0, hb0, hv10, hv20, sth[5 * W + c], sth[6 * W + c],
+                 sth[7 * W + c], sth[8 * W + c], z1, z2);
+        const unsigned g = (unsigned)ko * (unsigned)ny + (unsigned)gj;
+        stg2(y1 + g, z1.x, z1.y);
+        stg2(y2 + g, z2.x, z2.y);
+      }
+      tm = t0; t0 = t1; u0 = u1;
+      a0 = a1; b0 = b1; v10 = v11; v20 = v21; a1 = a2; b1 = b2; v11 = v12; v21 = v22;
+      ie1 = ie2;
+      xc = xn;
+      htm = ht0; ht0 = ht1; hu0 = hu1;
+      ha0 = ha1; hb0 = hb1; hv10 = hv11; hv20 = hv21; ha1 = ha2; hb1 = hb2; hv11 = w1; hv21 = w2;
+      hie1 = hie2;
+      hxc = hxn;
+      __syncthreads();
+      // every thread is done with the stage of step j - 2: refill it with the rows of step j + 2
+      if (j >= 2 && j + 2 < nsteps) issue(j + 2);
     }
   }
 }

@@ -119,6 +119,7 @@ class BatchSolver {
     TransferArgs tr;  // to the next coarser level
     const TransferArgs *tr_dev = nullptr;  // device copy of tr
     int rr_rows = 0;  // coarse rows per CTA of the fused residual + restriction (csrc/march2_tma.cuh); 0: separate kernels
+    int pj_rows = 0;  // rows per CTA of the fused prolongation + two sweeps (csrc/march2_tma.cuh); 0: separate kernels
   };
 
   BatchSolver(Arena &arena, cudaStream_t stream, const b200ms_options &opt) : arena_(arena), st_(stream), opt_(opt) {
@@ -476,8 +477,8 @@ class BatchSolver {
     dinv_ready_ = true;
     CUDA_CHECK(cudaStreamSynchronize(st_));
     CUDA_CHECK(cudaGetLastError());
-    prime_march2();
     plan_fused_tail();
+    prime_march2();
     capture_precondition_graph();
   }
 
@@ -627,6 +628,7 @@ class BatchSolver {
       for (size_t l = 0; l < lv.size(); ++l) {
         Level &v = lv[l];
         v.rr_rows = 0;
+        v.pj_rows = 0;
         if (!march2_eligible(v)) continue;
         int W = 0, nstrips = 0;
         march2_strips(v.ny, W, nstrips);
@@ -635,6 +637,7 @@ class BatchSolver {
           if (p.fn) march2_resident(p, md, W);
         }
         if (l + 1 < lv.size()) v.rr_rows = resid_restrict_plan((int)l, W, nstrips);
+        if (l + 1 < lv.size()) v.pj_rows = fused_post_plan((int)l, W, nstrips);
       }
     }
   }
@@ -716,6 +719,65 @@ class BatchSolver {
       if (best < 0 || cost < best * 0.999) { best = cost; best_ncr = ncr; }
     }
     return best_ncr;
+  }
+  // Rows per CTA of the fused post-smoothing pass on level l (csrc/march2_tma.cuh MODE_PROLONG_JACOBI2), or 0 where the
+  // prolongation and the two sweeps stay separate kernels: transfer_vec bit 3, V(2,2) cycles, the TMA pair kernel in one strip,
+  // a level of the explicit V-cycle (not the coarsest one, not in the fused tail) whose ring fits the shared memory of an SM.
+  // Where it applies, the results are those of the separate kernels, bit for bit.
+  int fused_post_plan(int l, int W, int nstrips) {
+    const Level &v = lv[l];
+    if (!(opt_.transfer_vec & 8) || opt_.mg_nu != 2 || opt_.mg_nu_growth != 0 || nstrips != 1 || v.ny > 2 * kM2MaxW) return 0;
+    if (l + 1 >= (int)lv.size() || (fused_l0_ >= 0 && l >= fused_l0_)) return 0;
+    if (march2_pick(MODE_JACOBI_D, v.ny).stages == 0 || v.tr.nxf != v.nx || v.tr.nyf != v.ny) return 0;
+    const size_t smem = pj_smem(W, v.tr.nyc);
+    const long key = -1 - ((long)W * 4096 + v.tr.nyc);  // (negative keys: this kernel's occupancy per width and coarse row)
+    auto it = m2_resident_.find(key);
+    if (it == m2_resident_.end()) {
+      int per_sm = 0;
+      CUDA_CHECK(cudaFuncSetAttribute(stencil_prolong_jacobi2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pj_smem(kM2MaxW, 2 * kM2MaxW)));
+      CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, stencil_prolong_jacobi2_kernel, W, smem));
+      it = m2_resident_.emplace(key, per_sm * sms_).first;
+    }
+    if (it->second < 1) return 0;
+    if (opt_.stencil_pair_rows > 0) return std::min(kM2MaxSteps - 6, 6 * ((opt_.stencil_pair_rows + 5) / 6));
+    // rows = 6 m, rows + 6 row steps per CTA: minimise (waves of resident CTAs) x (row steps per CTA + prologue), as march2_rows
+    int best_rows = 6;
+    double best = -1.0;
+    for (int rows = 6; rows + 6 <= kM2MaxSteps; rows += 6) {
+      const double waves = std::ceil((double)((v.nx + rows - 1) / rows) * B / it->second);
+      const double cost = waves * (rows + 6 + 5);
+      if (best < 0 || cost < best * 0.999 || (cost <= best * 1.001 && rows > best_rows && rows <= v.nx)) { best = cost; best_rows = rows; }
+      if (rows >= v.nx) break;
+    }
+    return best_rows;
+  }
+  // bit l set: level l runs its post-smoothing as one fused pass
+  int fused_post_levels() const {
+    int m = 0;
+    for (size_t l = 0; l < lv.size() && l < 16; ++l)
+      if (lv[l].pj_rows > 0) m |= 1 << l;
+    return m;
+  }
+  // y = two stored-diagonal sweeps on rhs from x + P lv[l + 1].x (y != x)
+  void prolong_jacobi2(int l, const P *x, const P *rhs, P *y) {
+    if constexpr (std::is_same<P, float>::value && std::is_same<PC, float>::value) {
+      const Level &v = lv[l];
+      StencilArgs<P, PC> a;
+      a.nx = v.nx; a.ny = v.ny; a.x = x; a.rhs = rhs; a.y = y;
+      a.fields = v.fields; a.field_bstride = v.fbstride; a.sigma = sigma_p_; a.cx = v.cx; a.cy = v.cy;
+      a.omega = opt_.mg_omega;
+      a.dinv = v.dinv;
+      a.tr = v.tr_dev;
+      a.coarse = lv[l + 1].x;
+      int W = 0, nstrips = 0;
+      march2_strips(v.ny, W, nstrips);
+      const dim3 grd(1, (v.nx + v.pj_rows - 1) / v.pj_rows, B);
+      const size_t smem = pj_smem(W, v.tr.nyc);
+      stencil_prolong_jacobi2_kernel<<<grd, W, smem, st_>>>(a, v.pj_rows);
+      if (l == 0) stats.stencil_applies += 2;
+      stats.launches++;
+      last_m2_ = M2Launch{stencil_prolong_jacobi2_kernel, grd, W, smem, a, v.pj_rows, stats.launches};
+    }
   }
   // bit l set: level l restricts its residual inside the residual kernel
   int resid_restrict_levels() const {
@@ -1144,24 +1206,33 @@ class BatchSolver {
       stats.launches++;
     }
     vcycle(l + 1, lv[l + 1].b, nullptr);
-    {
-      const TransferArgs &t = v.tr;
-      stats.launches++;
-      if (t.nyf >= 256 && opt_.transfer_tiled != 2) {  // four fine columns per thread
-        dim3 blk(64, 4), grd((t.nyf + 255) / 256, (t.nxf + 3) / 4, 2 * B);
-        if ((opt_.transfer_vec & 1) && std::is_same<P, float>::value && (t.nyf % 4) == 0) prolong_add4_kernel<P, true><<<grd, blk, 0, st_>>>(t, lv[l + 1].x, cur);
-        else prolong_add4_kernel<P, false><<<grd, blk, 0, st_>>>(t, lv[l + 1].x, cur);
-      } else {
-        dim3 blk(64, 4), grd((t.nyf + 63) / 64, (t.nxf + 3) / 4, 2 * B);
-        prolong_add_kernel<P><<<grd, blk, 0, st_>>>(t, lv[l + 1].x, cur);
-      }
+    if (v.pj_rows > 0) {  // prolongation and both post-smoothing sweeps in one pass (nu == 2)
+      P *dst = out ? out : oth;
+      prolong_jacobi2(l, cur, rin, dst);
+      if (!out) { v.x = dst; v.tmp = cur; }
+      return;
     }
+    prolong_add(l, cur);
     for (int s = 0; s < nu; ++s) {
       P *dst = (s == nu - 1 && out) ? out : oth;
       sweep(dst);
       if (dst != out) std::swap(cur, oth);
     }
     if (!out) { v.x = cur; v.tmp = oth; }
+  }
+
+  // fine += P lv[l + 1].x on level l
+  void prolong_add(int l, P *fine) {
+    const TransferArgs &t = lv[l].tr;
+    stats.launches++;
+    if (t.nyf >= 256 && opt_.transfer_tiled != 2) {  // four fine columns per thread
+      dim3 blk(64, 4), grd((t.nyf + 255) / 256, (t.nxf + 3) / 4, 2 * B);
+      if ((opt_.transfer_vec & 1) && std::is_same<P, float>::value && (t.nyf % 4) == 0) prolong_add4_kernel<P, true><<<grd, blk, 0, st_>>>(t, lv[l + 1].x, fine);
+      else prolong_add4_kernel<P, false><<<grd, blk, 0, st_>>>(t, lv[l + 1].x, fine);
+    } else {
+      dim3 blk(64, 4), grd((t.nyf + 63) / 64, (t.nxf + 3) / 4, 2 * B);
+      prolong_add_kernel<P><<<grd, blk, 0, st_>>>(t, lv[l + 1].x, fine);
+    }
   }
 
   // -- coarsest-level Krylov solve (indefinite shifts): GMRES(kc), Jacobi right-preconditioned, CGS2, run entirely
