@@ -29,7 +29,7 @@
 extern "C" {
 #endif
 
-#define B200MS_VERSION 210
+#define B200MS_VERSION 211
 
 /* return codes */
 enum {
@@ -92,7 +92,7 @@ typedef struct {
   /* ---- since version 205 ---- */
   const double *deps_table; /* NULL (nondispersive media), or nmedia x 9 complex128 (re,im): d eps / df (1/Hz) of each medium at this
                               problem's frequency, rasterised like eps_table; only the material term of result.dn_dfreq reads it
-                              (diagonal components) */
+                              (the diagonal components for diagonal problems, all nine for tensorial ones) */
   /* ---- since version 206 ---- */
   const double *d2eps_table; /* NULL, or nmedia x 9 complex128 (re,im): d^2 eps / df^2 (1/Hz^2) of each medium at this problem's
                               frequency, rasterised like eps_table; only result.d2n_dfreq2 reads it (diagonal components) */
@@ -144,12 +144,20 @@ typedef struct {
                             The trapezoid weights of flux, TE fraction and modal overlaps are then truncated to the part of each
                             cell the plane covers, like the reference's _diff_area (monitor_data.py:437-455: mid-points and end
                             points clipped to monitor.bounds).  Only the post-processing results depend on it */
-  const double *eps_dfreq; /* since version 205.  NULL (nondispersive medium), or d eps_cross / df (1/Hz) in the layout of `eps`; only the
-                            diagonal components are read, and only by the material term of result.dn_dfreq */
+  const double *eps_dfreq; /* since version 205.  NULL (nondispersive medium), or d eps_cross / df (1/Hz) in the layout of `eps`; read only
+                            by the material term of result.dn_dfreq: the diagonal components for diagonal problems, all nine for
+                            tensorial ones (left_solve) */
   const double *eps_d2freq; /* since version 206.  NULL, or d^2 eps_cross / df^2 (1/Hz^2) in the layout of `eps`; only the diagonal
                             components are read, and only by result.d2n_dfreq2 */
   const double *eps_d3freq; /* since version 210.  NULL, or d^3 eps_cross / df^3 (1/Hz^3) in the layout of `eps`; only the diagonal
                             components are read, and only by result.d3n_dfreq3 */
+  int left_solve;        /* since version 211.  1: a tensorial problem (angled plane, off-diagonal eps or mu) that asks for
+                            result.dn_dfreq / dn_deps_tensor is served by a second Krylov-Schur eigen-solve with the transposed operator
+                            (its left eigenvectors; about the cost of one more eigen-solve, see DESIGN.md §4) instead of being rejected.
+                            The whole device batch takes part; n_complex, the fields and the forward counters do not change.  With it,
+                            a tensorial problem may ask for dn_dfreq and dn_deps_tensor only (d2n_dfreq2, d2n_residual,
+                            d2n_dfreq_deps, d3n_dfreq3: B200MS_ERR_UNSUPPORTED; the three-component dn_deps: B200MS_ERR_ARG).  No
+                            effect on diagonal problems.  The relative solver and removed PEC unknowns stay unsupported */
 } b200ms_problem;
 
 typedef struct {
@@ -184,11 +192,13 @@ typedef struct {
   double total_ms;       /* out: host wall time of that batch incl. upload of the operator and download of the fields */
   double max_residual;   /* out: max_i ||A v_i - lambda_i v_i|| / (|lambda_i| ||v_i||) */
   /* ---- since version 205: first-order derivatives of each mode from its own solve (left eigenvector w = G J Q v, see DESIGN.md §4).
-     Diagonal problems only (PML, bend, lossy, both wall types, diagonal mu); asking for them on a tensorial, relative or
-     removed-PEC-unknown problem sets status B200MS_ERR_UNSUPPORTED.  They do not change which problems share a device batch,
-     nor n_complex or the fields ---- */
+     Diagonal problems (PML, bend, lossy, both wall types, diagonal mu), and since version 211 tensorial ones with
+     problem.left_solve; asking for them on a tensorial problem without left_solve, or on a relative or removed-PEC-unknown
+     problem, sets status B200MS_ERR_UNSUPPORTED.  They do not change which problems share a device batch, nor n_complex or the
+     fields ---- */
   double *dn_dfreq;      /* NULL, or caller-allocated num_modes complex128 (re,im): d(n_eff + i k_eff)/df (1/Hz), including the material
-                            dispersion given by problem.eps_dfreq / section.deps_table.  Group index: n_g = n_eff + f Re(dn/df) */
+                            dispersion given by problem.eps_dfreq / section.deps_table.  Group index: n_g = n_eff + f Re(dn/df).
+                            Tensorial problems (left_solve): NaN for a mode whose left eigenvector was not paired (see left_paired) */
   double *dn_deps;       /* NULL, or caller-allocated 3*nx*ny*num_modes complex128 (re,im), [xx|yy|zz][ix][iy][mode]: d(n_eff + i k_eff)
                             / d eps_aa of the caller's eps_cross at the Ex / Ey / Ez site of each cell (PML stretch held fixed; 0 at
                             PEC-valued cells); HOST or DEVICE memory like `fields` */
@@ -217,6 +227,20 @@ typedef struct {
   double *d3n_dfreq3;    /* NULL, or caller-allocated num_modes complex128 (re,im): d^3(n_eff + i k_eff)/df^3 (1/Hz^3), including the
                             material dispersion of problem.eps_dfreq / eps_d2freq / eps_d3freq (section: deps_table / d2eps_table /
                             d3eps_table).  NaN for a mode whose correction solve stopped above 100 x inner_tol */
+  /* ---- since version 211: the full-tensor permittivity gradient, and the pairing of left and right eigenvectors ---- */
+  double *dn_deps_tensor; /* NULL, or caller-allocated 9*nx*ny*num_modes complex128 (re,im), [xx|xy|xz|yx|yy|yz|zx|zy|zz][ix][iy][mode]
+                            (the eps_cross component order): d(n_eff + i k_eff) / d eps_ab of the caller's eps_cross at fixed PML
+                            stretch and fixed mu; HOST or DEVICE memory like `fields`.  Tensorial problems (left_solve): all nine
+                            rows, taken through the angle / bend congruence eps' = J eps J^T / det J; entries of eps' that the PEC
+                            model replaces give 0, and a mode whose left eigenvector was not paired gives NaN.  Diagonal problems:
+                            rows xx / yy / zz are those of dn_deps bit for bit and the six off-diagonal rows are 0 -- the reference
+                            solves such a problem as a diagonal one, and its n does not depend on off-diagonal components below
+                            the tensorial threshold.  Not together with dn_deps on a tensorial problem (B200MS_ERR_ARG) */
+  int left_paired;       /* out: -1 when none of dn_dfreq, dn_deps, dn_deps_tensor, d2n_dfreq2, d2n_dfreq_deps, d3n_dfreq3 is asked
+                            for; else the number of modes whose left eigenvector is known: num_modes for diagonal problems (it
+                            follows from the structure of the operator), and for tensorial ones the modes whose transposed Ritz
+                            value n_L was paired one-to-one with the mode's n (|n_L - n| <= 1e-6 |n|, both solves converged) and
+                            whose unit left / right vectors w, u have |w^T u| >= 1e-8 */
 } b200ms_result;
 
 /* Tunables (all have defaults; see DESIGN.md). */

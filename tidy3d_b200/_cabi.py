@@ -17,7 +17,7 @@ import numpy as np
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("B200MS_LIB") or os.path.join(_HERE, "libb200ms.so")  # B200MS_LIB: developer override (A/B of builds)
 
-ABI_VERSION = 210  # B200MS_VERSION of include/b200ms.h
+ABI_VERSION = 211  # B200MS_VERSION of include/b200ms.h
 OK, ERR_SHAPE, ERR_NO_MODES, ERR_UNSUPPORTED, ERR_CUDA, ERR_NOCONV, ERR_ARG = range(7)
 SPEC_NAMES = {0: "diagonal", 1: "tensorial_real", 2: "tensorial_complex"}
 
@@ -39,6 +39,7 @@ class Problem(C.Structure):
         ("angle_theta", C.c_double), ("angle_phi", C.c_double),
         ("eps", _dp), ("coords_x", _dp), ("coords_y", _dp), ("mu", _dp), ("section", C.POINTER(SectionStruct)), ("basis_e", _dp),
         ("grid_correction", _dp), ("plane_bounds", _dp), ("eps_dfreq", _dp), ("eps_d2freq", _dp), ("eps_d3freq", _dp),
+        ("left_solve", C.c_int),
     ]  # fmt: skip
 
 
@@ -48,6 +49,7 @@ class Result(C.Structure):
         ("outer_iters", C.c_int), ("op_applies", C.c_int), ("inner_iters", C.c_int), ("stencil_applies", C.c_int),
         ("is_complex", C.c_int), ("solve_ms", C.c_double), ("total_ms", C.c_double), ("max_residual", C.c_double),
         ("dn_dfreq", _dp), ("dn_deps", _dp), ("d2n_dfreq2", _dp), ("d2n_residual", _dp), ("d2n_dfreq_deps", _dp), ("d3n_dfreq3", _dp),
+        ("dn_deps_tensor", _dp), ("left_paired", C.c_int),
     ]  # fmt: skip
 
 
@@ -137,7 +139,7 @@ class PackedProblem:
 
     def __init__(self, eps_cross, coords, freq, mode_spec, symmetry=(0, 0), direction="+", eps_packed=None, basis_fields=None,
                  mu_cross=None, target_override=None, incidence=False, post=0, section=None, grid_correction=None, plane_bounds=None,
-                 eps_dfreq=None, derivatives=False, eps_d2freq=None, second=False, eps_d3freq=None, third=False):
+                 eps_dfreq=None, derivatives=False, eps_d2freq=None, second=False, eps_d3freq=None, third=False, left_solve=False):
         self.section = None
         if section is not None:  # geometric cross-section rasterised on the device (tidy3d_b200/sections.py); no eps array
             self.section, self._section_arrays = section.pack(float(freq), (len(coords[0]) - 1, len(coords[1]) - 1), dispersion=derivatives,
@@ -255,6 +257,7 @@ class PackedProblem:
             if self.eps_d3freq.shape != (9, self.nx, self.ny):
                 raise ValueError("eps_d3freq must have the nine components and the shape of eps_cross")
             p.eps_d3freq = _ptr(self.eps_d3freq.view(np.float64))
+        p.left_solve = 1 if left_solve else 0
         self.struct = p
         self.num_modes = p.num_modes
 
@@ -346,7 +349,7 @@ class Handle:
             pass
 
     def solve_batch(self, packed, want_fields=True, fields_ptrs=None, want_flux=False, want_overlaps=False, want_dfreq=False, want_deps=False,
-                    want_d2freq=False, want_group_eps=False, want_d3freq=False):
+                    want_d2freq=False, want_group_eps=False, want_d3freq=False, want_deps_tensor=False):
         """packed: list of PackedProblem.  Returns (rc, fields list | None, n_complex list, Result structs).
 
         ``fields_ptrs``: optional list of raw addresses (host or DEVICE memory, e.g. ``tensor.data_ptr()``) the library
@@ -355,7 +358,10 @@ class Handle:
         ``want_deps``: d n / df and d n / d eps of every mode (``last_dn_dfreq`` / ``last_dn_deps``); ``want_d2freq``: d^2 n / df^2 and
         the residual of its correction solve (``last_d2n_dfreq2`` / ``last_d2n_residual``); ``want_group_eps``: d(dn/df) / d eps of
         every mode from that correction solve (``last_d2n_dfreq_deps``); ``want_d3freq``: d^3 n / df^3 of every mode from the same
-        correction solve (``last_d3n_dfreq3``)."""
+        correction solve (``last_d3n_dfreq3``); ``want_deps_tensor``: the nine-component d n / d eps of every mode (result.dn_deps_tensor,
+        (9, nx, ny, M) arrays in ``last_dn_deps``; not together with ``want_deps``)."""
+        if want_deps and want_deps_tensor:
+            raise ValueError("want_deps and want_deps_tensor fill the same list: ask for one of them")
         n = len(packed)
         probs = (Problem * n)(*[p.struct for p in packed])
         results = (Result * n)()
@@ -374,6 +380,10 @@ class Handle:
                 d = np.zeros((3, p.nx, p.ny, p.num_modes), dtype=np.complex128)
                 self.last_dn_deps.append(d)
                 results[i].dn_deps = _ptr(d.view(np.float64))
+            if want_deps_tensor:
+                d = np.zeros((9, p.nx, p.ny, p.num_modes), dtype=np.complex128)
+                self.last_dn_deps.append(d)
+                results[i].dn_deps_tensor = _ptr(d.view(np.float64))
             if want_d2freq:
                 d, r = np.zeros(p.num_modes, dtype=np.complex128), np.zeros(p.num_modes)
                 self.last_d2n_dfreq2.append(d)

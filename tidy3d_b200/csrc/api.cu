@@ -225,6 +225,11 @@ GroupKey group_key(const ProblemSetup &s, const b200ms_problem &p) {
 
 inline size_t align256(size_t n) { return (n + 255) & ~size_t(255); }
 
+// a result that asks for any mode derivative
+inline bool asks_derivatives(const b200ms_result &r) {
+  return r.dn_dfreq || r.dn_deps || r.dn_deps_tensor || r.d2n_dfreq2 || r.d2n_dfreq_deps || r.d3n_dfreq3;
+}
+
 // A window of consecutive problems whose raw media are resident on the device: set-up stages A-C of host_setup.hpp with
 // the per-cell work (reductions) done by medium_scan_kernel.
 struct Window {
@@ -708,16 +713,17 @@ bool batch_refs(const Window &W, const std::vector<int> &ids, std::vector<const 
   return share;
 }
 
-// The diagonal (xx, yy, zz) of a per-problem input in the layout of `eps` -- the caller's array `arr(p)`, or for a section the
-// rasteriser fed with the per-medium table `tab(sec)` -- into dst [B][3][N], zero where a problem has neither.  `scratch` holds
-// one rasterised section (9 N complex values, then the section upload); the stream is synchronised after every problem.
+// The diagonal (xx, yy, zz; ncomp = 3) or all nine components (ncomp = 9) of a per-problem input in the layout of `eps` -- the
+// caller's array `arr(p)`, or for a section the rasteriser fed with the per-medium table `tab(sec)` -- into dst [B][ncomp][N],
+// zero where a problem has neither.  `scratch` holds one rasterised section (9 N complex values, then the section upload); the
+// stream is synchronised after every problem.
 template <typename Arr, typename Tab>
 void gather_diag(b200ms_handle *h, const std::vector<int> &ids, const Window &W, const b200ms_problem *prob, int nx, int ny, Arr arr,
-                 Tab tab, cplx *dst, unsigned char *scratch) {
+                 Tab tab, cplx *dst, unsigned char *scratch, int ncomp = 3) {
   const int B = (int)ids.size();
   const size_t N = (size_t)nx * ny;
   cudaStream_t st = h->stream;
-  CUDA_CHECK(cudaMemsetAsync(dst, 0, (size_t)B * 3 * N * sizeof(cplx), st));
+  CUDA_CHECK(cudaMemsetAsync(dst, 0, (size_t)B * ncomp * N * sizeof(cplx), st));
   for (int b = 0; b < B; ++b) {
     const b200ms_problem &p = prob[W.i0 + ids[b]];
     const cplx *src = nullptr;
@@ -732,8 +738,11 @@ void gather_diag(b200ms_handle *h, const std::vector<int> &ids, const Window &W,
       src = full;
     }
     if (!src) continue;
-    for (int a = 0; a < 3; ++a)
-      CUDA_CHECK(cudaMemcpyAsync(dst + ((size_t)b * 3 + a) * N, src + (size_t)(4 * a) * N, N * sizeof(cplx), cudaMemcpyDefault, st));
+    if (ncomp == 9)
+      CUDA_CHECK(cudaMemcpyAsync(dst + (size_t)b * 9 * N, src, 9 * N * sizeof(cplx), cudaMemcpyDefault, st));
+    else
+      for (int a = 0; a < 3; ++a)
+        CUDA_CHECK(cudaMemcpyAsync(dst + ((size_t)b * 3 + a) * N, src + (size_t)(4 * a) * N, N * sizeof(cplx), cudaMemcpyDefault, st));
     CUDA_CHECK(cudaStreamSynchronize(st));  // the section scratch is reused by the next problem
   }
 }
@@ -761,7 +770,7 @@ void derivative_pass(b200ms_handle *h, BatchSolver<T, C, P, PC> &S, const std::v
   bool any_map = false, any_disp = false;
   for (int b = 0; b < B; ++b) {
     const b200ms_problem &p = prob[W.i0 + ids[b]];
-    any_map = any_map || res[W.i0 + ids[b]].dn_deps;
+    any_map = any_map || res[W.i0 + ids[b]].dn_deps || res[W.i0 + ids[b]].dn_deps_tensor;
     any_disp = any_disp || (p.eps ? p.eps_dfreq != nullptr : p.section->deps_table != nullptr);
   }
   // host tables: f dc/df = -c kappa / s (kappa / s = Re(l) / l for the stretched length l = s dl k0), metric lengths
@@ -797,7 +806,8 @@ void derivative_pass(b200ms_handle *h, BatchSolver<T, C, P, PC> &S, const std::v
   auto arr1 = [](const b200ms_problem &p) { return p.eps_dfreq; };
   auto tab1 = [](const b200ms_section &sec) { return sec.deps_table; };
   const size_t sec_bytes = gather_scratch_bytes(ids, W, prob, nx, ny, tab1);
-  const size_t o_sec = o_map + (any_map ? align256((size_t)B * 3 * N * k * sizeof(cplx)) : 0);
+  const size_t o_zero = o_map + (any_map ? align256((size_t)B * 3 * N * k * sizeof(cplx)) : 0);  // zero rows of dn_deps_tensor
+  const size_t o_sec = o_zero + (any_map ? align256(N * k * sizeof(cplx)) : 0);
   h->deriv.reserve(o_sec + sec_bytes + 256);
   unsigned char *base = h->deriv.p;
   cudaStream_t st = h->stream;
@@ -857,12 +867,180 @@ void derivative_pass(b200ms_handle *h, BatchSolver<T, C, P, PC> &S, const std::v
   else deriv_map_kernel<T, C, false><<<grd, blk, 0, st>>>(a);
   CUDA_CHECK(cudaGetLastError());
   h->stats.launches += 1;
+  const cplx *zero = reinterpret_cast<const cplx *>(base + o_zero);
+  CUDA_CHECK(cudaMemsetAsync(base + o_zero, 0, N * k * sizeof(cplx), st));
   for (int b = 0; b < B; ++b) {
     b200ms_result &r = res[W.i0 + ids[b]];
     if (r.dn_deps)
       CUDA_CHECK(cudaMemcpyAsync(r.dn_deps, a.map + (size_t)b * 3 * N * k, 3 * N * k * sizeof(cplx), cudaMemcpyDefault, st));
+    if (r.dn_deps_tensor)  // rows xx, yy, zz of the nine-row layout; the off-diagonal rows are 0
+      for (int c = 0; c < 9; ++c)
+        CUDA_CHECK(cudaMemcpyAsync(reinterpret_cast<cplx *>(r.dn_deps_tensor) + (size_t)c * N * k,
+                                   c % 4 == 0 ? a.map + ((size_t)b * 3 + c / 4) * N * k : zero, N * k * sizeof(cplx), cudaMemcpyDefault, st));
   }
   CUDA_CHECK(cudaStreamSynchronize(st));
+}
+
+// Left eigenvectors of a tensorial batch (problems that ask for derivatives with left_solve): the transposed Krylov-Schur pass.
+// Call with the sorted right Ritz vectors in S.ritz_ptr(); they are kept in S.right_ptr().  Mode q of problem b is paired with
+// the transposed Ritz value nearest its n (the model's eigenpairs rule) when that assignment is one-to-one within the problem
+// and |n_L - n_q| <= 1e-6 |n_q| (and both solves converged); the w^T u test follows in the scan (tensor_derivative_pass).
+// Leaves the paired left vectors in S.ritz_ptr() in the sorted order (zero vectors for unpaired modes) and returns the pairing.
+template <typename T, typename C, typename P, typename PC>
+std::vector<char> left_vectors(b200ms_handle *h, BatchSolver<T, C, P, PC> &S, const std::vector<const ProblemSetup *> &ps,
+                               const std::vector<cd> &nsorted, const std::vector<int> &fwd_nconv) {
+  const int B = S.B, k = S.k;
+  S.keep_right();
+  typename BatchSolver<T, C, P, PC>::EigResult e;
+  {
+    NvtxRange r("b200ms:transposed eigen-iteration");
+    e = S.solve_transposed();
+  }
+  std::vector<int> src((size_t)B * k, -1);
+  std::vector<char> paired((size_t)B * k, 0);
+  double worst = 0.0;
+  for (int b = 0; b < B; ++b) {
+    if (fwd_nconv[b] != k || e.nconv[b] != k) continue;
+    std::vector<cd> nl(k);
+    for (int j = 0; j < k; ++j) {
+      const cd th = e.theta[(size_t)b * k + j];
+      nl[j] = std::abs(th) > 0 ? ps[b]->sigma_t + 1.0 / th : cd(NAN, NAN);
+    }
+    std::vector<int> pick(k), uses(k, 0);
+    for (int q = 0; q < k; ++q) {
+      const cd n = nsorted[(size_t)b * k + q];
+      int best = 0;
+      for (int j = 1; j < k; ++j)
+        if (std::abs(nl[j] - n) < std::abs(nl[best] - n)) best = j;
+      pick[q] = best;
+      uses[best]++;
+    }
+    for (int q = 0; q < k; ++q) {
+      const cd n = nsorted[(size_t)b * k + q];
+      const double rel = std::abs(nl[pick[q]] - n) / std::abs(n);
+      worst = std::max(worst, rel);
+      if (uses[pick[q]] == 1 && rel <= 1e-6) {
+        src[(size_t)b * k + q] = pick[q];
+        paired[(size_t)b * k + q] = 1;
+      }
+    }
+  }
+  S.permute_ritz(src);
+  if (h->opt.verbose) fprintf(stderr, "[b200ms] transposed solve: largest |n_L - n| / |n| %.2e\n", worst);
+  return paired;
+}
+
+// Derivative pass of a tensorial device batch (csrc/derivatives.cuh tensor_deriv_*) after left_vectors: result.dn_dfreq and
+// result.dn_deps_tensor (and left_paired) of the problems that ask for them.  d_refs / share: the batch's raw media as
+// BatchSolver::build received them.
+template <typename T, typename C, typename P, typename PC>
+void tensor_derivative_pass(b200ms_handle *h, BatchSolver<T, C, P, PC> &S, const std::vector<const ProblemSetup *> &ps, const std::vector<int> &ids,
+                            const Window &W, const b200ms_problem *prob, b200ms_result *res, const std::vector<char> &paired,
+                            const MediumRef *d_refs, bool share) {
+  if constexpr (std::is_same<T, cplx>::value) {
+    const int B = (int)ids.size(), k = S.k, nx = S.nx, ny = S.ny;
+    const size_t N = (size_t)nx * ny;
+    bool any_map = false, any_disp = false;
+    for (int b = 0; b < B; ++b) {
+      const b200ms_problem &p = prob[W.i0 + ids[b]];
+      any_map = any_map || res[W.i0 + ids[b]].dn_deps_tensor;
+      any_disp = any_disp || (p.eps ? p.eps_dfreq != nullptr : p.section->deps_table != nullptr);
+    }
+    // host tables c +- f dc/df (f dc/df = -c kappa / s, as derivative_pass)
+    std::vector<cplx> cxp((size_t)B * 4 * nx), cxm(cxp.size()), cyp((size_t)B * 4 * ny), cym(cyp.size());
+    for (int b = 0; b < B; ++b)
+      for (int a = 0; a < 2; ++a) {
+        const Axis &A = ps[b]->ax[a];
+        const int n = A.n;
+        std::vector<cd> c;
+        A.coefficients(c);
+        cplx *cp = (a == 0 ? cxp.data() : cyp.data()) + (size_t)b * 4 * n, *cm = (a == 0 ? cxm.data() : cym.data()) + (size_t)b * 4 * n;
+        for (int i = 0; i < n; ++i) {
+          const cd rf = A.lf[i].real() / A.lf[i], rb = A.lb[i].real() / A.lb[i];
+          for (int w = 0; w < 4; ++w) {
+            const cd c0 = c[(size_t)w * n + i], dc = -c0 * (w < 2 ? rf : rb);
+            cp[(size_t)w * n + i] = mk((c0 + dc).real(), (c0 + dc).imag());
+            cm[(size_t)w * n + i] = mk((c0 - dc).real(), (c0 - dc).imag());
+          }
+        }
+      }
+    const size_t bx = align256(cxp.size() * sizeof(cplx)), by = align256(cyp.size() * sizeof(cplx));
+    const size_t o_cxp = 0, o_cxm = bx, o_cyp = 2 * bx, o_cym = 2 * bx + by, o_part = 2 * bx + 2 * by;
+    const int nch = (int)std::min<size_t>(kDerivChunks, (N + 255) / 256);
+    const size_t o_sum = o_part + align256((size_t)B * k * nch * 3 * sizeof(cplx)), o_scale = o_sum + align256((size_t)B * k * 3 * sizeof(cplx));
+    const size_t o_deps = o_scale + align256((size_t)B * k * sizeof(cplx));
+    const size_t o_map = o_deps + (any_disp ? align256((size_t)B * 9 * N * sizeof(cplx)) : 0);
+    auto arr1 = [](const b200ms_problem &p) { return p.eps_dfreq; };
+    auto tab1 = [](const b200ms_section &sec) { return sec.deps_table; };
+    const size_t sec_bytes = gather_scratch_bytes(ids, W, prob, nx, ny, tab1);
+    const size_t o_sec = o_map + (any_map ? align256((size_t)B * 9 * N * k * sizeof(cplx)) : 0);
+    h->deriv.reserve(o_sec + sec_bytes + 256);
+    unsigned char *base = h->deriv.p;
+    cudaStream_t st = h->stream;
+    CUDA_CHECK(cudaMemcpyAsync(base + o_cxp, cxp.data(), cxp.size() * sizeof(cplx), cudaMemcpyHostToDevice, st));
+    CUDA_CHECK(cudaMemcpyAsync(base + o_cxm, cxm.data(), cxm.size() * sizeof(cplx), cudaMemcpyHostToDevice, st));
+    CUDA_CHECK(cudaMemcpyAsync(base + o_cyp, cyp.data(), cyp.size() * sizeof(cplx), cudaMemcpyHostToDevice, st));
+    CUDA_CHECK(cudaMemcpyAsync(base + o_cym, cym.data(), cym.size() * sizeof(cplx), cudaMemcpyHostToDevice, st));
+    cplx *deps = reinterpret_cast<cplx *>(base + o_deps);
+    if (any_disp) gather_diag(h, ids, W, prob, nx, ny, arr1, tab1, deps, base + o_sec, 9);  // d eps / df, [B][9][N]
+    TensorDerivArgs<C> a;
+    a.nx = nx; a.ny = ny; a.num_modes = k; a.u = S.right_ptr(); a.w = S.ritz_ptr(); a.vstride = S.vstride;
+    a.ft = S.tensor_fields(); a.ft_bstride = S.shared_fields ? 0 : 18 * N; a.cx = S.lv[0].cx_true; a.cy = S.lv[0].cy_true;
+    a.cxp = reinterpret_cast<const cplx *>(base + o_cxp); a.cxm = reinterpret_cast<const cplx *>(base + o_cxm);
+    a.cyp = reinterpret_cast<const cplx *>(base + o_cyp); a.cym = reinterpret_cast<const cplx *>(base + o_cym);
+    a.med = d_refs; a.med_bstride = share ? 0 : 1;
+    a.deps = any_disp ? deps : nullptr;
+    a.msign = S.msign_;
+    a.partial = reinterpret_cast<cplx *>(base + o_part);
+    a.scale = reinterpret_cast<const cplx *>(base + o_scale);
+    a.map = any_map ? reinterpret_cast<cplx *>(base + o_map) : nullptr;
+    cplx *dsum = reinterpret_cast<cplx *>(base + o_sum);
+    {
+      NvtxRange r("b200ms:tensorial derivative pass");
+      tensor_deriv_scan_kernel<C><<<dim3(nch, B * k), 256, 0, st>>>(a);
+      deriv_final_kernel<<<(B * k * 3 + 127) / 128, 128, 0, st>>>(a.partial, nch, B * k * 3, dsum);
+      CUDA_CHECK(cudaGetLastError());
+    }
+    std::vector<cplx> sums((size_t)B * k * 3);
+    CUDA_CHECK(cudaMemcpyAsync(sums.data(), dsum, sums.size() * sizeof(cplx), cudaMemcpyDeviceToHost, st));
+    CUDA_CHECK(cudaStreamSynchronize(st));
+    h->stats.launches += 2;
+    // dn/df = knorm [msign (-i) w^T (f dM/df) u / f + sum_g d n/d eps . d eps/df] / w^T u; w, u are unit vectors (Ritz vectors)
+    std::vector<cplx> scale((size_t)B * k);
+    double smallest = 1e300;
+    for (int b = 0; b < B; ++b) {
+      const b200ms_problem &p = prob[W.i0 + ids[b]];
+      b200ms_result &r = res[W.i0 + ids[b]];
+      int np = 0;
+      for (int q = 0; q < k; ++q) {
+        const cplx *sq = sums.data() + ((size_t)b * k + q) * 3;
+        const cd wu(sq[0].re, sq[0].im), da(sq[1].re, sq[1].im), mat(sq[2].re, sq[2].im);
+        const bool ok = paired[(size_t)b * k + q] && std::abs(wu) >= 1e-8;
+        if (paired[(size_t)b * k + q]) smallest = std::min(smallest, std::abs(wu));
+        np += ok ? 1 : 0;
+        const cd sc = ok ? ps[b]->knorm / wu : cd(NAN, NAN);
+        scale[(size_t)b * k + q] = mk(sc.real(), sc.imag());
+        const cd dn = sc * (cd(0, -S.msign_) * da / p.freq + mat);
+        if (r.dn_dfreq) {
+          r.dn_dfreq[2 * q] = dn.real();
+          r.dn_dfreq[2 * q + 1] = dn.imag();
+        }
+      }
+      r.left_paired = np;
+    }
+    if (h->opt.verbose) fprintf(stderr, "[b200ms] transposed solve: smallest paired |w^T u| %.2e\n", smallest);
+    if (!any_map) return;
+    CUDA_CHECK(cudaMemcpyAsync(base + o_scale, scale.data(), scale.size() * sizeof(cplx), cudaMemcpyHostToDevice, st));
+    tensor_deriv_map_kernel<C><<<dim3((ny + 63) / 64, (nx + 3) / 4, B * k), dim3(64, 4), 0, st>>>(a);
+    CUDA_CHECK(cudaGetLastError());
+    h->stats.launches += 1;
+    for (int b = 0; b < B; ++b) {
+      b200ms_result &r = res[W.i0 + ids[b]];
+      if (r.dn_deps_tensor)
+        CUDA_CHECK(cudaMemcpyAsync(r.dn_deps_tensor, a.map + (size_t)b * 9 * N * k, 9 * N * k * sizeof(cplx), cudaMemcpyDefault, st));
+    }
+    CUDA_CHECK(cudaStreamSynchronize(st));
+  }
 }
 
 
@@ -1144,6 +1322,13 @@ void solve_group(b200ms_handle *h, const std::vector<int> &ids, const Window &W,
   BatchSolver<T, C, P, PC> S(h->arena, h->stream, h->opt);
   auto wall0 = std::chrono::steady_clock::now();
   S.single_out_ = prob[W.i0 + ids[0]].precision == 1;
+  // a tensorial batch in which some problem asks for derivatives with left_solve: the whole batch also runs the transposed solve
+  bool left = false;
+  for (int b = 0; b < B; ++b) {
+    const b200ms_result &rb = res[W.i0 + ids[b]];
+    left = left || (ps[b]->tensorial && prob[W.i0 + ids[b]].left_solve && (rb.dn_dfreq || rb.dn_deps_tensor));
+  }
+  S.pairing_ = left;
   const MediumRef *d_refs = upload_refs(h, refs, h->stream);
   {
     NvtxRange r("b200ms:build (hierarchy, coefficient fields, graph capture)");
@@ -1230,13 +1415,18 @@ void solve_group(b200ms_handle *h, const std::vector<int> &ids, const Window &W,
     h->warm_B = B; h->warm_k = k; h->warm_len = S.len; h->warm_tsize = (int)sizeof(T);
     h->warm_valid = true;
   }
+  // the forward solve's counters, before any derivative pass runs more solves in this batch
+  const SolveStats fwd = S.stats;
   bool want_deriv = false, want_disp = false;
   for (int b = 0; b < B; ++b) {
     const b200ms_result &rb = res[W.i0 + ids[b]];
-    want_deriv = want_deriv || rb.dn_dfreq || rb.dn_deps || rb.d2n_dfreq2 || rb.d2n_dfreq_deps || rb.d3n_dfreq3;
+    want_deriv = want_deriv || asks_derivatives(rb);
     want_disp = want_disp || rb.d2n_dfreq2 || rb.d2n_dfreq_deps || rb.d3n_dfreq3;
   }
-  if (want_deriv) {
+  if (left) {
+    const std::vector<char> paired = left_vectors(h, S, ps, nsorted, eig.nconv);
+    tensor_derivative_pass(h, S, ps, ids, W, prob, res, paired, d_refs, share);
+  } else if (want_deriv) {
     DerivArgs<T, C> da;
     derivative_pass(h, S, ps, ids, W, prob, res, nsorted, da);
     if (want_disp) dispersion_pass(h, S, ps, ids, W, prob, res, nsorted, lam, da);
@@ -1265,10 +1455,12 @@ void solve_group(b200ms_handle *h, const std::vector<int> &ids, const Window &W,
     }
     r.eps_spec = ps[b]->eps_spec;
     r.converged = eig.nconv[b];
-    r.outer_iters = S.stats.restarts;
-    r.op_applies = S.stats.op_applies;
-    r.inner_iters = S.stats.inner_iters;
-    r.stencil_applies = (int)std::min<long>(S.stats.launches, 2147483647L);
+    r.outer_iters = fwd.restarts;
+    r.op_applies = fwd.op_applies;
+    r.inner_iters = fwd.inner_iters;
+    r.stencil_applies = (int)std::min<long>(fwd.launches, 2147483647L);
+    if (!asks_derivatives(r)) r.left_paired = -1;
+    else if (!S.tensor_) r.left_paired = k;
     r.is_complex = real_arith ? 0 : 1;
     r.solve_ms = ms;
     r.total_ms = total_ms;
@@ -1278,21 +1470,22 @@ void solve_group(b200ms_handle *h, const std::vector<int> &ids, const Window &W,
     // screened for garbage (O(1)) here.
     // With PEC-valued cells (|eps| = 1e8) that amplification makes the figure meaningless at the reference's tolerance
     // (measured 0.25 on pec_block_40 with |dn| < 1e-8), so the screen is skipped there.
-    r.status = (relative || (eig.nconv[b] == k && eig.ok && (maxres[b] < 1e-1 || ps[b]->has_pec) && S.stats.inner_failures == 0)) ? B200MS_OK : B200MS_ERR_NOCONV;
+    r.status = (relative || (eig.nconv[b] == k && eig.ok && (maxres[b] < 1e-1 || ps[b]->has_pec) && fwd.inner_failures == 0)) ? B200MS_OK : B200MS_ERR_NOCONV;
     if (h->opt.verbose)
       fprintf(stderr, "[b200ms] prob %d: conv %d/%d ok %d restarts %d op %d inner %d cycles %d syncs %ld reorth %d innerfail %d res %.2e ms %.1f\n", W.i0 + ids[b],
-              eig.nconv[b], k, (int)eig.ok, S.stats.restarts, S.stats.op_applies, S.stats.inner_iters, S.stats.inner_cycles, S.stats.host_syncs,
-              S.stats.outer_second_pass, S.stats.inner_failures, maxres[b], ms);
+              eig.nconv[b], k, (int)eig.ok, fwd.restarts, fwd.op_applies, fwd.inner_iters, fwd.inner_cycles, fwd.host_syncs,
+              fwd.outer_second_pass, fwd.inner_failures, maxres[b], ms);
   }
 }
 
-// device memory one problem of a batch needs in the solver arena (Krylov bases dominate)
-size_t bytes_per_problem(const ProblemSetup &s, const b200ms_options &opt) {
+// device memory one problem of a batch needs in the solver arena (Krylov bases dominate); left: the batch keeps its k right Ritz
+// vectors through a transposed solve (BatchSolver::pairing_)
+size_t bytes_per_problem(const ProblemSetup &s, const b200ms_options &opt, bool left) {
   const size_t N = (size_t)s.nx * s.ny;
   const size_t len = (s.tensorial ? 4 : 2) * N;
   const size_t sv = s.is_complex ? 16 : 8;
   const int m = opt.ncv > 0 ? opt.ncv : std::max(2 * s.num_modes + 1, 20);
-  size_t vecs = (m + 1) + (2 * opt.gmres_restart + 1) + 4 + s.num_modes;
+  size_t vecs = (m + 1) + (2 * opt.gmres_restart + 1) + 4 + s.num_modes * (left ? 2 : 1);
   size_t bytes = vecs * len * sv;
   bytes += (size_t)7 * 2 * N * sv * 4 / 3;            // multigrid level work vectors (x, b, r, tmp, dinv + coarse levels)
   bytes += (size_t)(s.has_mu ? 6 : 3) * N * 16 * 2;   // coefficient fields in both precisions
@@ -1365,6 +1558,7 @@ extern "C" int b200ms_solve_batch(b200ms_handle *h, int nprob, const b200ms_prob
         for (int i = i0; i < i1; ++i) {
           res[i].status = res[i].n_complex ? B200MS_OK : B200MS_ERR_ARG;
           res[i].converged = 0;
+          res[i].left_paired = -1;
         }
         std::map<GroupKey, std::vector<int>> groups;
         size_t out_bytes = 0;
@@ -1375,11 +1569,22 @@ extern "C" int b200ms_solve_batch(b200ms_handle *h, int nprob, const b200ms_prob
           res[i].eps_spec = s.eps_spec;
           res[i].is_complex = s.is_complex;
           std::string err = s.error;
-          if (res[i].status == B200MS_OK && (res[i].dn_dfreq || res[i].dn_deps || res[i].d2n_dfreq2 || res[i].d2n_dfreq_deps || res[i].d3n_dfreq3) && (s.tensorial || s.relative || s.masked)) {
+          const bool left = prob[i].left_solve != 0;
+          if (res[i].status == B200MS_OK && asks_derivatives(res[i]) && ((s.tensorial && !left) || s.relative || s.masked)) {
             res[i].status = B200MS_ERR_UNSUPPORTED;
-            err = s.tensorial ? "mode derivatives: tensorial problems (angled planes, off-diagonal eps) are not supported"
+            err = (s.tensorial && !left) ? "mode derivatives: tensorial problems (angled planes, off-diagonal eps) need the transposed eigen-solve: "
+                                           "set b200ms_problem.left_solve (Python: left_solve=True), about one more eigen-solve"
                   : s.relative ? "mode derivatives: the relative mode solver (basis fields) is not supported"
                                : "mode derivatives: removed PEC unknowns (mu_cross / split_curl_scaling with PEC cells) are not supported";
+          }
+          if (res[i].status == B200MS_OK && s.tensorial && left && (res[i].d2n_dfreq2 || res[i].d2n_residual || res[i].d2n_dfreq_deps || res[i].d3n_dfreq3)) {
+            res[i].status = B200MS_ERR_UNSUPPORTED;
+            err = "mode derivatives: tensorial problems give dn_dfreq and dn_deps_tensor only (higher frequency derivatives and the group-index "
+                  "gradient are not supported)";
+          }
+          if (res[i].status == B200MS_OK && s.tensorial && left && res[i].dn_deps) {
+            res[i].status = B200MS_ERR_ARG;
+            err = "mode derivatives: a tensorial problem's permittivity gradient has nine components: pass result.dn_deps_tensor, not dn_deps";
           }
           if (res[i].status == B200MS_OK && (prob[i].post || res[i].flux || res[i].te_fraction || res[i].overlap_prev) && s.num_modes > kPostMaxModes) {
             res[i].status = B200MS_ERR_ARG;
@@ -1403,7 +1608,9 @@ extern "C" int b200ms_solve_batch(b200ms_handle *h, int nprob, const b200ms_prob
         size_t cursor = 0;
         for (auto &kv : groups) {
           const std::vector<int> &all = kv.second;
-          const size_t per = bytes_per_problem(W.setups[all[0]], h->opt);
+          bool left = false;
+          for (int id : all) left = left || (W.setups[id].tensorial && prob[i0 + id].left_solve && (res[i0 + id].dn_dfreq || res[i0 + id].dn_deps_tensor));
+          const size_t per = bytes_per_problem(W.setups[all[0]], h->opt, left);
           int bmax = (int)std::max<size_t>(1, std::min<size_t>((size_t)std::max(1, h->opt.max_batch), (size_t)(0.8 * free_b) / per));
           for (size_t s0 = 0; s0 < all.size();) {
             std::vector<int> ids(all.begin() + s0, all.begin() + std::min(all.size(), s0 + bmax));
@@ -1778,7 +1985,8 @@ int debug_run(b200ms_handle *h, const Window &W, int what, int level, int mode, 
       h->err = "b200ms_debug_batch: what 3 / 4 (transposed operator / preconditioner) take tensorial problems, level 0 and mode 0 or 1";
       return B200MS_ERR_ARG;
     }
-    S.adjoint_ = true;
+    S.pairing_ = true;
+    S.transposed_ = true;
     what -= 3;
   }
   S.build(ps, share, upload_refs(h, refs, h->stream));

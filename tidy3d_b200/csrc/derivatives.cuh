@@ -7,6 +7,7 @@
 // [A(c + dc) v - A(c - dc) v] / 2 with dc = f dc/df = -c kappa / s.
 #pragma once
 #include "kernels.cuh"
+#include "medium.cuh"
 
 namespace b200ms {
 
@@ -667,6 +668,144 @@ __global__ void __launch_bounds__(256) third_scan_kernel(DispArgs<T, C> a, Third
     __syncthreads();
   }
   if (threadIdx.x < 6) t.partial[(((size_t)b * 2 + threadIdx.x / 3) * gridDim.x + blockIdx.x) * 3 + threadIdx.x % 3] = red[threadIdx.x][0];
+}
+
+// ------------------------------------------------------------------------------------------------
+// Tensorial problems: first-order derivatives of the eigenvalue n of mat = msign (-i) M (oracle/tensor_derivatives.py is the
+// float64 model) from the sorted right Ritz vectors u and the left ones w of the transposed Krylov-Schur pass, paired mode by
+// mode (api.cu).  dn = msign (-i) w^T (dM) u / w^T u.  M has degree <= 2 in the 1-D coefficients, so f dM/df u is exactly
+// [M(c + c') - M(c - c')] u / 2; M is affine in the per-site derived fields q of eps' (ft_[0..8]), and the nine
+// sensitivities w^T (dM/dq_j) u at a site are the 16 block terms of _eps_terms, which collapse to products of the dual
+// intermediate Ub = Dxf^T w1 + Dyf^T w2 (of w), K = Dxb u4 - Dyb u3 (of u) and the site values:
+//   (q0, q1, q2) <- (-Ub u1, -Ub u2, Ub K),  q3 <- w3 K,  q4 <- -w4 K,  (S_xx, S_xy) <- (-w4 u1, -w4 u2),  (S_yx, S_yy) <- (w3 u1, w3 u2).
+// They are chained through dq/dt' written in q alone (1/t_zz = q2, t_zx/t_zz = q0, t_zy/t_zz = q1, t_yz/t_zz = q3,
+// t_xz/t_zz = q4), the PEC model (entries of eps' that are PEC-valued, as tensor_fields_kernel finds them: 0) and the
+// congruence eps' = J eps J^T / det J back to the caller's eps_cross: g = J^T g' J / det J.
+// ------------------------------------------------------------------------------------------------
+template <typename C>
+struct TensorDerivArgs {
+  int nx, ny, num_modes;
+  const cplx *u, *w;             // sorted right Ritz vectors and the paired left ones: slot q of problem b at q vstride + b 4N
+  size_t vstride;
+  const C *ft;                   // [fb][18][N] derived coefficient fields
+  size_t ft_bstride;
+  const cplx *cx, *cy;           // [B][4][n] 1-D coefficients
+  const cplx *cxp, *cyp, *cxm, *cym;  // [B][4][n] c + f dc/df and c - f dc/df
+  const MediumRef *med;          // raw media (PEC marker, congruence), problem b at med[b * med_bstride]
+  int med_bstride;
+  const cplx *deps;              // [B][9][N] d eps_cross / df (1/Hz) in the eps_cross component order, or null
+  double msign;
+  cplx *partial;                 // [B*M][nchunk][3]
+  const cplx *scale;             // [B][M]: map = gradient numerator * scale
+  cplx *map;                     // [B][9][N][M]
+};
+
+template <typename C>
+__device__ __forceinline__ TensorCell<C> tensor_deriv_cell(const TensorDerivArgs<C> &a, const cplx *vec, int b, int m, const cplx *cx, const cplx *cy) {
+  const size_t N = (size_t)a.nx * a.ny;
+  const cplx *v = vec + (size_t)m * a.vstride + (size_t)b * 4 * N;
+  return TensorCell<C>{v, v + N, v + 2 * N, v + 3 * N, a.ft + a.ft_bstride * b, cx + (size_t)b * 4 * a.nx, cy + (size_t)b * 4 * a.ny, a.nx, a.ny, N};
+}
+
+// w^T (d mat / d eps_cross[k](i, j)) u, k in the eps_cross order (not yet divided by w^T u)
+template <typename C>
+__device__ __forceinline__ void tensor_eps_grad(const TensorDerivArgs<C> &a, const TensorCell<C> &tu, const TensorCell<C> &tw, int b, int i, int j,
+                                                cplx g[9]) {
+  const size_t s = (size_t)i * a.ny + j;
+  const cplx mi = mk(0.0, -a.msign);
+  const cplx ub = mi * tw.Ub(i, j), kk = tu.K(i, j);
+  const cplx u1 = ldg(tu.ex + s), u2 = ldg(tu.ey + s), w3 = mi * ldg(tw.hx + s), w4 = mi * ldg(tw.hy + s);
+  const cplx q0 = to_cplx(tu.F(0, i, j)), q1 = to_cplx(tu.F(1, i, j)), q2 = to_cplx(tu.F(2, i, j));
+  const cplx q3 = to_cplx(tu.F(3, i, j)), q4 = to_cplx(tu.F(4, i, j));
+  cplx gt[9];  // d/d eps'_ab, row-major
+  for (int k = 0; k < 9; ++k) gt[k] = mk(0.0, 0.0);
+  const cplx c0 = -(ub * u1), c1 = -(ub * u2), c2 = ub * kk, c3 = w3 * kk, c4 = -(w4 * kk);
+  gt[6] = c0 * q2;
+  gt[7] = c1 * q2;
+  gt[5] = c3 * q2;
+  gt[2] = c4 * q2;
+  gt[8] = -(q2 * (c0 * q0 + c1 * q1 + c2 * q2 + c3 * q3 + c4 * q4));
+  const cplx cs[4] = {-(w4 * u1), -(w4 * u2), w3 * u1, w3 * u2};  // S_xx, S_xy, S_yx, S_yy
+  const cplx qa[2] = {q4, q3}, qz[2] = {q0, q1};                 // t_az / t_zz, t_zb / t_zz
+  for (int r = 0; r < 2; ++r)
+    for (int c = 0; c < 2; ++c) {
+      const cplx v = cs[2 * r + c];
+      gt[3 * r + c] += v;
+      gt[3 * r + 2] -= v * qz[c];
+      gt[6 + c] -= v * qa[r];
+      gt[8] += v * (qa[r] * qz[c]);
+    }
+  // the raw congruence at this cell, as tensor_fields_kernel forms it before the PEC model
+  const MediumRef &r = a.med[(size_t)b * a.med_bstride];
+  const double de = r.p.norm_axis >= 0 ? r.p.de[r.p.norm_axis == 0 ? i : j] : 1.0;
+  cplx et[9], mt[9];
+  cell_tensors(r.eps, nullptr, (size_t)a.nx * a.ny, s, r.p.a, r.p.b, de, 1.0, et, mt);
+  for (int k = 0; k < 9; ++k)
+    if (is_pec_val(et[k])) gt[k] = mk(0.0, 0.0);
+  const double J[3][3] = {{1, 0, r.p.a}, {0, 1, r.p.b}, {0, 0, de}};
+  for (int c = 0; c < 3; ++c)
+    for (int d = 0; d < 3; ++d) {
+      cplx acc = mk(0.0, 0.0);
+      for (int p = 0; p < 3; ++p)
+        for (int q = 0; q < 3; ++q)
+          if (J[p][c] != 0.0 && J[q][d] != 0.0) acc += (J[p][c] * J[q][d]) * gt[3 * p + q];
+      g[3 * c + d] = cdivd(acc, de);
+    }
+}
+
+// grid (nchunk, B*M), 256 threads: partial sums of w^T u, w^T [M(c + c') - M(c - c')] u / 2 and the material term per chunk
+template <typename C>
+__global__ void __launch_bounds__(256) tensor_deriv_scan_kernel(TensorDerivArgs<C> a) {
+  const int M = a.num_modes, bm = blockIdx.y, b = bm / M, m = bm % M;
+  const int ny = a.ny;
+  const size_t N = (size_t)a.nx * ny;
+  const TensorCell<C> tu = tensor_deriv_cell(a, a.u, b, m, a.cx, a.cy), tw = tensor_deriv_cell(a, a.w, b, m, a.cx, a.cy);
+  const TensorCell<C> tp = tensor_deriv_cell(a, a.u, b, m, a.cxp, a.cyp), tm = tensor_deriv_cell(a, a.u, b, m, a.cxm, a.cym);
+  const cplx *de = a.deps ? a.deps + (size_t)b * 9 * N : nullptr;
+  cplx s_wu = mk(0.0, 0.0), s_da = mk(0.0, 0.0), s_mat = mk(0.0, 0.0);
+  for (size_t g = (size_t)blockIdx.x * 256 + threadIdx.x; g < N; g += (size_t)gridDim.x * 256) {
+    const int i = (int)(g / ny), j = (int)(g % ny);
+    const cplx u0 = ldg(tu.ex + g), u1 = ldg(tu.ey + g), u2 = ldg(tu.hx + g), u3 = ldg(tu.hy + g);
+    const cplx w0 = ldg(tw.ex + g), w1 = ldg(tw.ey + g), w2 = ldg(tw.hx + g), w3 = ldg(tw.hy + g);
+    s_wu += w0 * u0 + w1 * u1 + w2 * u2 + w3 * u3;
+    cplx p[4], q[4];
+    tp.apply(i, j, u0, u1, u2, u3, p[0], p[1], p[2], p[3]);
+    tm.apply(i, j, u0, u1, u2, u3, q[0], q[1], q[2], q[3]);
+    s_da += 0.5 * (w0 * (p[0] - q[0]) + w1 * (p[1] - q[1]) + w2 * (p[2] - q[2]) + w3 * (p[3] - q[3]));
+    if (de) {
+      cplx gr[9];
+      tensor_eps_grad(a, tu, tw, b, i, j, gr);
+      for (int k = 0; k < 9; ++k) s_mat += gr[k] * ldg(de + (size_t)k * N + g);
+    }
+  }
+  __shared__ cplx red[3][256];
+  red[0][threadIdx.x] = s_wu;
+  red[1][threadIdx.x] = s_da;
+  red[2][threadIdx.x] = s_mat;
+  __syncthreads();
+  for (int h = 128; h > 0; h >>= 1) {
+    if ((int)threadIdx.x < h)
+      for (int k = 0; k < 3; ++k) red[k][threadIdx.x] += red[k][threadIdx.x + h];
+    __syncthreads();
+  }
+  if (threadIdx.x < 3) a.partial[((size_t)bm * gridDim.x + blockIdx.x) * 3 + threadIdx.x] = red[threadIdx.x][0];
+}
+
+// grid like epilogue_kernel: map[b][k][g][m] = (w^T d mat / d eps_cross[k](g) u) * scale[b][m]
+template <typename C>
+__global__ void __launch_bounds__(256) tensor_deriv_map_kernel(TensorDerivArgs<C> a) {
+  const int nx = a.nx, ny = a.ny, M = a.num_modes;
+  const size_t N = (size_t)nx * ny;
+  const int j = blockIdx.x * 64 + threadIdx.x, i = blockIdx.y * 4 + threadIdx.y;
+  const int m = blockIdx.z % M, b = blockIdx.z / M;
+  if (i >= nx || j >= ny) return;
+  const TensorCell<C> tu = tensor_deriv_cell(a, a.u, b, m, a.cx, a.cy), tw = tensor_deriv_cell(a, a.w, b, m, a.cx, a.cy);
+  cplx gr[9];
+  tensor_eps_grad(a, tu, tw, b, i, j, gr);
+  const cplx sc = a.scale[(size_t)b * M + m];
+  const size_t g = (size_t)i * ny + j;
+  cplx *o = a.map + (size_t)b * 9 * N * M;
+  for (int k = 0; k < 9; ++k) o[((size_t)k * N + g) * M + m] = gr[k] * sc;
 }
 
 }  // namespace b200ms

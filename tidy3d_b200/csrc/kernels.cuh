@@ -1271,6 +1271,16 @@ struct TensorCell {
     if (i < 0 || j < 0 || i >= nx || j >= ny) return mk(0.0, 0.0);
     return F(11, i, j) * Tb(i, j) + F(12, i, j) * ld(ex, i, j) - F(13, i, j) * ld(ey, i, j);
   }
+  // (M [Ex;Ey;Hx;Hy]) at (i, j), given the site's own four values
+  __device__ __forceinline__ void apply(int i, int j, cplx ex0, cplx ey0, cplx hx0, cplx hy0, cplx &r1, cplx &r2, cplx &r3, cplx &r4) const {
+    const cplx u00 = U(i, j), u10 = U(i + 1, j), u01 = U(i, j + 1);
+    const cplx t00 = Tt(i, j), tm0 = Tt(i - 1, j), t0m = Tt(i, j - 1);
+    const cplx kk = K(i, j), gg = G(i, j);
+    r1 = CX(0, i) * u00 + CX(1, i) * u10 + F(12, i, j) * gg + F(16, i, j) * hx0 + F(17, i, j) * hy0;
+    r2 = CY(0, j) * u00 + CY(1, j) * u01 - F(13, i, j) * gg - F(14, i, j) * hx0 - F(15, i, j) * hy0;
+    r3 = CX(2, i) * t00 + CX(3, i) * tm0 + F(3, i, j) * kk + F(7, i, j) * ex0 + F(8, i, j) * ey0;
+    r4 = CY(2, j) * t00 + CY(3, j) * t0m - F(4, i, j) * kk - F(5, i, j) * ex0 - F(6, i, j) * ey0;
+  }
 };
 
 // y = (mat - sigma) w  or  rhs - (mat - sigma) w;  TR: the same with mat^T = msign (-i) M^T (left eigenvectors)
@@ -1294,13 +1304,7 @@ __global__ void __launch_bounds__(256) tensor_apply_kernel(TensorArgs<C> a) {
     r3 = -(t.F(9, i, j) * tb) - (t.CY(2, j) * k00 + t.CY(3, j + 1) * k01) + t.F(16, i, j) * ex - t.F(14, i, j) * ey;
     r4 = -(t.F(10, i, j) * tb) + (t.CX(2, i) * k00 + t.CX(3, i + 1) * k10) + t.F(17, i, j) * ex - t.F(15, i, j) * ey;
   } else {
-    const cplx u00 = t.U(i, j), u10 = t.U(i + 1, j), u01 = t.U(i, j + 1);
-    const cplx t00 = t.Tt(i, j), tm0 = t.Tt(i - 1, j), t0m = t.Tt(i, j - 1);
-    const cplx kk = t.K(i, j), gg = t.G(i, j);
-    r1 = t.CX(0, i) * u00 + t.CX(1, i) * u10 + t.F(12, i, j) * gg + t.F(16, i, j) * hx + t.F(17, i, j) * hy;
-    r2 = t.CY(0, j) * u00 + t.CY(1, j) * u01 - t.F(13, i, j) * gg - t.F(14, i, j) * hx - t.F(15, i, j) * hy;
-    r3 = t.CX(2, i) * t00 + t.CX(3, i) * tm0 + t.F(3, i, j) * kk + t.F(7, i, j) * ex + t.F(8, i, j) * ey;
-    r4 = t.CY(2, j) * t00 + t.CY(3, j) * t0m - t.F(4, i, j) * kk - t.F(5, i, j) * ex - t.F(6, i, j) * ey;
+    t.apply(i, j, ex, ey, hx, hy, r1, r2, r3, r4);
   }
   const cplx mi = mk(0.0, -a.msign);  // msign * (-i)
   const cplx sg = ldg(a.sigma + b);

@@ -133,9 +133,12 @@ class BatchSolver {
   bool tensor_ = false;
   bool masked_ = false;      // incidence-matrix formulation: unknowns marked by exx == 0 / eyy == 0 are held at zero
   bool single_out_ = false;  // fields are delivered as complex64 (mode_spec.precision == "single")
-  // tensorial, set before build(): the Krylov-side operator and the preconditioner act with mat^T (left eigenvectors); only
-  // such a batch allocates and uploads the pairing metric and the +sigma scalars of precondition_tensor_T
-  bool adjoint_ = false;
+  // tensorial, set before build(): the batch allocates and uploads the pairing metric and the +sigma scalars of
+  // precondition_tensor_T, and room for the k sorted right Ritz vectors (keep_right); forward batches without it allocate,
+  // upload and compute exactly what they did before
+  bool pairing_ = false;
+  // tensorial, run time (needs pairing_): the Krylov-side operator and the preconditioner act with mat^T (left eigenvectors)
+  bool transposed_ = false;
   double msign_ = 1.0;
   bool has_mu = false, shared_fields = false;
   std::vector<Level> lv;
@@ -238,10 +241,11 @@ class BatchSolver {
     if (tensor_) {
       sz.add<C>(fB * 18 * N);
       sz.add<T>(vsE * 6);
-      sz.add<cplx>((size_t)B * (adjoint_ ? 16 : 8));
-      if (adjoint_) {
+      sz.add<cplx>((size_t)B * (pairing_ ? 16 : 8));
+      if (pairing_) {
         sz.add<cplx>((size_t)B * 2 * nx);
         sz.add<cplx>((size_t)B * 2 * ny);
+        sz.add<T>((size_t)k * vstride);
       }
     }
     coarse_krylov_ = kh_limit > 0.0;
@@ -402,7 +406,7 @@ class BatchSolver {
     if (tensor_) {
       ft_ = arena_.get<C>(fB * 18 * N);
       for (int q = 0; q < 6; ++q) tb_[q] = arena_.get<T>(vsE);
-      tcoef_ = arena_.get<cplx>((size_t)B * (adjoint_ ? 16 : 8));
+      tcoef_ = arena_.get<cplx>((size_t)B * (pairing_ ? 16 : 8));
       {
         dim3 grd((unsigned)std::min<size_t>((N + 255) / 256, 2048), (unsigned)fB);
         tensor_fields_kernel<C><<<grd, 256, 0, st_>>>(d_refs, ft_, (size_t)18 * N);
@@ -412,17 +416,18 @@ class BatchSolver {
       // per-problem scalars of the preconditioner: [0] -sigma_t, [1] i*msign, [2] 1/s, [3] -1/s, [4] 1  (s = -sigma_t^2);
       // adjoint batch: at 8 B the same set for the shift +sigma_t, which the transposed preconditioner inverts through (s does
       // not change)
-      std::vector<cplx> hc((size_t)B * (adjoint_ ? 16 : 8));
+      std::vector<cplx> hc((size_t)B * (pairing_ ? 16 : 8));
       for (int b = 0; b < B; ++b) {
         const cd st = ps[b]->sigma_t, sd = -st * st;
         const cd v[5] = {-st, cd(0, msign_), 1.0 / sd, -1.0 / sd, cd(1, 0)};
         for (int q = 0; q < 5; ++q) {
           hc[(size_t)q * B + b] = mk(v[q].real(), v[q].imag());
-          if (adjoint_) hc[(size_t)(8 + q) * B + b] = q == 0 ? mk(st.real(), st.imag()) : hc[(size_t)q * B + b];
+          if (pairing_) hc[(size_t)(8 + q) * B + b] = q == 0 ? mk(st.real(), st.imag()) : hc[(size_t)q * B + b];
         }
       }
       CUDA_CHECK(cudaMemcpyAsync(tcoef_, hc.data(), hc.size() * sizeof(cplx), cudaMemcpyHostToDevice, st_));
-      if (adjoint_) {
+      if (pairing_) {
+        right_ = arena_.get<T>((size_t)k * vstride);
         // metric of the pairing K (tensor_pair_kernel): complex-stretched primal / dual lengths, the first dual cell halved at a
         // PMC wall
         tgx_ = arena_.get<cplx>((size_t)B * 2 * nx);
@@ -882,7 +887,7 @@ class BatchSolver {
         a.ft = ft_; a.ft_bstride = shared_fields ? 0 : 18 * N; a.cx = lv[0].cx_true; a.cy = lv[0].cy_true;
         a.sigma = sigma_; a.msign = msign_;
         dim3 blk(64, 4), grd((ny + 63) / 64, (nx + 3) / 4, B);
-        if (adjoint_) tensor_apply_kernel<C, true><<<grd, blk, 0, st_>>>(a);
+        if (transposed_) tensor_apply_kernel<C, true><<<grd, blk, 0, st_>>>(a);
         else tensor_apply_kernel<C, false><<<grd, blk, 0, st_>>>(a);
         stats.launches++;
         return;
@@ -966,7 +971,7 @@ class BatchSolver {
   // residual), converting on the way in and out when the multigrid runs in fp32.  Two cycles per application roughly
   // halve the FGMRES iteration count, which pays because the Gram-Schmidt cost grows quadratically with it.
   void precondition(const T *v, T *z) {
-    if (tensor_ && adjoint_) {
+    if (tensor_ && transposed_) {
       precondition_tensor_T(v, z);
     } else if (tensor_) {
       precondition_tensor(v, z, tcoef_);
@@ -2203,6 +2208,35 @@ class BatchSolver {
   size_t output_bytes_per_problem() const { return (size_t)6 * N * k * (single_out_ ? sizeof(cplxf) : sizeof(cplx)); }
   T *hessenberg() { return Hd_; }
   T *ritz_ptr() { return ritz_; }
+  T *right_ptr() { return right_; }
+  const C *tensor_fields() const { return ft_; }
+
+  // ---- left eigenvectors of a tensorial batch (pairing_): the transposed Krylov-Schur pass ----
+  // keep the sorted right Ritz vectors (ritz_) where the transposed solve does not write
+  void keep_right() {
+    CUDA_CHECK(cudaMemcpyAsync(right_, ritz_, (size_t)k * vstride * sizeof(T), cudaMemcpyDeviceToDevice, st_));
+    CUDA_CHECK(cudaStreamSynchronize(st_));
+  }
+  // Krylov-Schur with mat^T at the forward shift and k, from the forward solve's seeded start vector: the spectrum of mat^T is
+  // that of mat, so the wanted set is the same k eigenvalues.  Ritz values and vectors (wanted order) as krylov_schur leaves them.
+  EigResult solve_transposed() {
+    transposed_ = true;
+    init_start_vector(0);
+    EigResult e = krylov_schur(false);
+    transposed_ = false;
+    return e;
+  }
+  // ritz_ slot q of problem b <- old slot src[b k + q]; src < 0 gives a zero vector
+  void permute_ritz(const std::vector<int> &src) {
+    std::vector<T> ph((size_t)B * k * k, zero_of<T>());
+    for (int b = 0; b < B; ++b)
+      for (int q = 0; q < k; ++q)
+        if (src[(size_t)b * k + q] >= 0) ph[((size_t)b * k + src[(size_t)b * k + q]) * k + q] = from_real<T>(1.0);
+    CUDA_CHECK(cudaMemcpyAsync(qbuf_, ph.data(), ph.size() * sizeof(T), cudaMemcpyHostToDevice, st_));
+    lincomb(ritz_, vstride, qbuf_, k, k, k, Zg_, vstride);
+    CUDA_CHECK(cudaMemcpyAsync(ritz_, Zg_, (size_t)k * vstride * sizeof(T), cudaMemcpyDeviceToDevice, st_));
+    CUDA_CHECK(cudaStreamSynchronize(st_));
+  }
 
   // ---- b200ms_debug_krylov: one Krylov vector operation of this batch on caller data, through the member function the
   // solver runs, in the buffers it runs it in (include/b200ms.h documents what / nv / the arrays).  U: T, or P for the
@@ -2441,6 +2475,7 @@ class BatchSolver {
   C *ft_ = nullptr;
   T *tb_[6] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
   cplx *tcoef_ = nullptr, *tgx_ = nullptr, *tgy_ = nullptr;
+  T *right_ = nullptr;  // pairing_ batches: the sorted right Ritz vectors while the transposed solve runs
   std::vector<cd> sig_mg_host_;
   bool dinv_ready_ = false;
   int sms_ = 0;  // streaming multiprocessors of the device

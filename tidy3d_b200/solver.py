@@ -78,7 +78,7 @@ def _undo_split_curl(fields, split):
 
 def compute_modes_batch(
     problems: Sequence[dict], device: int = -1, want_fields: bool = True, return_info: bool = False, handle=None,
-    fields_ptrs=None, post: Optional[Sequence[str]] = None, derivatives: Optional[Sequence[str]] = None,
+    fields_ptrs=None, post: Optional[Sequence[str]] = None, derivatives: Optional[Sequence[str]] = None, left_solve: bool = False,
 ):
     """Solve many independent mode problems in one device call.
 
@@ -118,6 +118,15 @@ def compute_modes_batch(
     ``d2n_dfreq2`` is), ``dispersion_slope`` (dD/d(wavelength), ps/(nm^2 km), ``plugin.dispersion_slope_of``) and ``beta3``
     (d^3 beta / d omega^3, ps^3/km, ``plugin.beta3_of``).  It implies ``"freq2"`` and ``"freq"``, whose outputs do not change;
     its material term also reads a problem's ``eps_d3freq=`` (d^3 eps_cross / df^3) or a section's callable media.
+
+    ``left_solve=True`` extends ``"freq"`` and ``"eps"`` to tensorial problems (angled planes, off-diagonal eps such as rotated
+    anisotropic crystals), which otherwise raise ``NotImplementedError``: their left eigenvectors come from a second eigen-solve
+    with the transposed operator, about the cost of one more solve per device batch that holds such a problem.  ``dn_deps`` is
+    then (9, Nx, Ny, M), d(n_eff + i k_eff) / d eps_ab of ``eps_cross`` in its component order (xx, xy, ..., zz) at fixed PML
+    stretch and mu; material dispersion reads all nine components of ``eps_dfreq=`` or of a section's callable media.  A mode whose
+    left eigenvector could not be paired with it gets NaN; ``left_paired`` in the info dict counts the modes that were (num_modes
+    for diagonal problems, -1 without derivatives).  Diagonal problems solve as without the flag and report ``dn_deps`` as
+    (3, Nx, Ny, M).  With it, ``"freq2"``, ``"group_eps"`` and ``"freq3"`` still raise on tensorial problems.
     """
     post = tuple(post or ())
     unknown = set(post) - {"gauge", "normalize", "flux", "overlaps"}
@@ -127,6 +136,8 @@ def compute_modes_batch(
     unknown = set(derivatives) - {"freq", "eps", "freq2", "group_eps", "freq3"}
     if unknown:
         raise ValueError(f"unknown derivative(s): {sorted(unknown)}")
+    if left_solve and not derivatives:
+        raise ValueError("left_solve=True serves derivatives=(\"freq\", \"eps\") of tensorial problems: ask for derivatives as well")
     group_eps = "group_eps" in derivatives
     if group_eps:
         derivatives = derivatives + tuple(d for d in ("eps", "freq2") if d not in derivatives)
@@ -161,7 +172,7 @@ def compute_modes_batch(
             incidence=(split is not None or p.get("mu_cross") is not None),  # solver.py:93
             post=post_flags, grid_correction=p.get("grid_correction"), plane_bounds=p.get("plane_bounds"),
             eps_dfreq=p.get("eps_dfreq"), derivatives="freq" in derivatives, eps_d2freq=p.get("eps_d2freq"), second=second,
-            eps_d3freq=p.get("eps_d3freq"), third=third,
+            eps_d3freq=p.get("eps_d3freq"), third=third, left_solve=left_solve,
         )  # fmt: skip
         if split is None and section is None:
             cache[key] = pk.eps
@@ -174,8 +185,9 @@ def compute_modes_batch(
         packed.append(pk)
     h = handle or get_handle(device)  # after input validation: argument errors do not need a GPU
     with h.lock:
-        dkw = dict(want_dfreq="freq" in derivatives, want_deps="eps" in derivatives, want_d2freq=second, want_group_eps=group_eps,
-                   want_d3freq=third) if derivatives else {}
+        want_eps = "eps" in derivatives
+        dkw = dict(want_dfreq="freq" in derivatives, want_deps=want_eps and not left_solve, want_deps_tensor=want_eps and left_solve,
+                   want_d2freq=second, want_group_eps=group_eps, want_d3freq=third) if derivatives else {}
         rc, fields, ncs, results = h.solve_batch(packed, want_fields, fields_ptrs, want_flux=("flux" in post or "normalize" in post),
                                                  want_overlaps="overlaps" in post, **dkw)
         flux_out, te_out, ov_out = h.last_flux, h.last_te, h.last_overlaps
@@ -197,7 +209,7 @@ def compute_modes_batch(
         infos.append(
             dict(converged=r.converged, restarts=r.outer_iters, op_applies=r.op_applies, inner_iters=r.inner_iters,
                  stencil_applies=r.stencil_applies, is_complex=bool(r.is_complex), solve_ms=r.solve_ms, total_ms=r.total_ms,
-                 max_residual=r.max_residual)
+                 max_residual=r.max_residual, left_paired=r.left_paired)
         )  # fmt: skip
         if flux_out:
             infos[-1]["flux"] = flux_out[i]
@@ -208,7 +220,8 @@ def compute_modes_batch(
             infos[-1]["dn_dfreq"] = dfreq_out[i]
             infos[-1]["n_group"] = ncs[i].real + float(packed[i].struct.freq) * dfreq_out[i].real
         if deps_out:
-            infos[-1]["dn_deps"] = deps_out[i]
+            # with left_solve the nine-row layout was asked for: diagonal problems report their xx / yy / zz rows
+            infos[-1]["dn_deps"] = deps_out[i][[0, 4, 8]] if (left_solve and r.eps_spec == 0) else deps_out[i]
         if d2_out:
             from .plugin import dispersion_of  # noqa: PLC0415  (plugin imports this module)
 
@@ -217,7 +230,7 @@ def compute_modes_batch(
             infos[-1]["dispersion"] = dispersion_of(float(packed[i].struct.freq), dfreq_out[i], d2_out[i])
         if gmap_out:
             infos[-1]["d2n_dfreq_deps"] = gmap_out[i]
-            infos[-1]["dng_deps"] = deps_out[i].real + float(packed[i].struct.freq) * gmap_out[i].real
+            infos[-1]["dng_deps"] = infos[-1]["dn_deps"].real + float(packed[i].struct.freq) * gmap_out[i].real
         if d3_out:
             from .plugin import beta3_of, dispersion_slope_of  # noqa: PLC0415  (plugin imports this module)
 
