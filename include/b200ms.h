@@ -243,6 +243,30 @@ typedef struct {
                             whose unit left / right vectors w, u have |w^T u| >= 1e-8 */
 } b200ms_result;
 
+/* ---- Fourth frequency derivative of each mode (b200ms_solve_batch_ext; the symbol is the capability, the version stays 211).
+   One more correction solve per mode, (A - lambda) x2 = -Pi [(A' - lambda') x + (A'' - lambda'') v / 2], and the structural
+   second-order left correction w_hat2 give lambda'''' exactly (the functional w^T A v / w^T v is stationary in both vectors):
+     lambda'''' w^T v = w^T A''''v + 4 w_hat^T A'''v + 4 w^T A'''x + 12 w_hat2^T A''v + 12 w^T A''x2 + 12 w_hat^T A''x
+                        + 24 w_hat2^T A'x + 24 w_hat^T A'x2 + 24 w_hat2^T (A - lambda) x2 - 24 lambda' D_3 - 12 lambda'' D_2 - 4 lambda''' D_1
+   in the scaled direction ' = f d/df (D_k: the t^k coefficient of (w + t w_hat + t^2 w_hat2)^T (v + t x + t^2 x2); see DESIGN.md §4).
+   Same scope as d3n_dfreq3, which it needs; n_complex, the fields and every other derivative do not change when it is asked
+   for.  Both arrays are indexed like prob / res. ---- */
+typedef struct {
+  const double *eps_d4freq;  /* NULL, or d^4 eps_cross / df^4 (1/Hz^4) in the layout of problem.eps; only the diagonal components
+                                are read, and only by d4n_dfreq4.  Not with problem.section */
+  const double *d4eps_table; /* NULL, or problem.section->nmedia x 9 complex128 (re,im): d^4 eps / df^4 (1/Hz^4) of each medium of
+                                the problem's section at its frequency, rasterised like eps_table (diagonal components) */
+} b200ms_problem_ext;
+
+typedef struct {
+  double *d4n_dfreq4;    /* NULL, or caller-allocated num_modes complex128 (re,im): d^4(n_eff + i k_eff)/df^4 (1/Hz^4), including the
+                            material dispersion of problem.eps_dfreq .. eps_d3freq and eps_d4freq (section: deps_table .. d3eps_table
+                            and d4eps_table).  Needs result.d3n_dfreq3 (else B200MS_ERR_ARG).  NaN for a mode whose first or second
+                            correction solve stopped above 100 x inner_tol.  beta4 (s^4/m) = (4 Re n''' + f Re n'''') / (8 pi^3 c) */
+  double *d4n_residual;  /* NULL, or caller-allocated num_modes doubles: final relative residual of each mode's second-order correction
+                            solve (needs d4n_dfreq4) */
+} b200ms_result_ext;
+
 /* Tunables (all have defaults; see DESIGN.md). */
 typedef struct {
   double eig_tol;        /* relative Ritz residual tolerance; default 1.19e-7 = the reference's ARPACK tol (solver.py:20,745);
@@ -343,6 +367,10 @@ void b200ms_host_free(void *ptr);
  * the device.  Returns B200MS_OK if every problem succeeded, else the first failing status (each
  * result carries its own status). */
 int b200ms_solve_batch(b200ms_handle *h, int nprob, const b200ms_problem *prob, b200ms_result *res);
+/* b200ms_solve_batch with the fourth frequency derivative: pext / rext are NULL or nprob entries each (b200ms_solve_batch is
+ * this call with both NULL). */
+int b200ms_solve_batch_ext(b200ms_handle *h, int nprob, const b200ms_problem *prob, b200ms_result *res, const b200ms_problem_ext *pext,
+                           const b200ms_result_ext *rext);
 
 /* Benchmark / roofline hook: run one of the two hot stencil kernels `nrep` times on `nbatch` device-resident copies
  * of the operator of `prob` and return the mean kernel time (CUDA events on the library stream).

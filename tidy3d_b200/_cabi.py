@@ -53,6 +53,14 @@ class Result(C.Structure):
     ]  # fmt: skip
 
 
+class ProblemExt(C.Structure):
+    _fields_ = [("eps_d4freq", _dp), ("d4eps_table", _dp)]
+
+
+class ResultExt(C.Structure):
+    _fields_ = [("d4n_dfreq4", _dp), ("d4n_residual", _dp)]
+
+
 class Options(C.Structure):
     _fields_ = [
         ("eig_tol", C.c_double), ("inner_tol", C.c_double), ("ncv", C.c_int), ("max_restarts", C.c_int),
@@ -73,7 +81,7 @@ class Stats(C.Structure):
 
 EXPORTS = [
     "b200ms_version", "b200ms_get_stats", "b200ms_default_options", "b200ms_create", "b200ms_destroy", "b200ms_set_options",
-    "b200ms_last_error", "b200ms_host_alloc", "b200ms_host_free", "b200ms_solve_batch", "b200ms_bench_stencil", "b200ms_debug_schur", "b200ms_debug_setup",
+    "b200ms_last_error", "b200ms_host_alloc", "b200ms_host_free", "b200ms_solve_batch", "b200ms_solve_batch_ext", "b200ms_bench_stencil", "b200ms_debug_schur", "b200ms_debug_setup",
     "b200ms_debug_hierarchy", "b200ms_debug_batch", "b200ms_debug_apply", "b200ms_debug_vcycle", "b200ms_debug_solve", "b200ms_debug_march2_geometry", "b200ms_debug_post_tables", "b200ms_debug_post_tables_bounded", "b200ms_debug_te_terms", "b200ms_debug_grid_factors", "b200ms_debug_krylov", "b200ms_debug_fields",
 ]  # fmt: skip
 
@@ -111,6 +119,8 @@ def lib():
             L.b200ms_host_free.argtypes = [C.c_void_p]
             L.b200ms_host_free.restype = None
             L.b200ms_solve_batch.argtypes = [C.c_void_p, C.c_int, C.POINTER(Problem), C.POINTER(Result)]
+            L.b200ms_solve_batch_ext.argtypes = [C.c_void_p, C.c_int, C.POINTER(Problem), C.POINTER(Result), C.POINTER(ProblemExt),
+                                                 C.POINTER(ResultExt)]
             L.b200ms_bench_stencil.argtypes = [C.c_void_p, C.POINTER(Problem), C.c_int, C.c_int, C.c_int, C.c_int, _dp, _dp, _dp, _dp]
             L.b200ms_debug_schur.argtypes = [C.c_int, _dp, _dp, _dp]
             L.b200ms_debug_setup.argtypes = [C.POINTER(Problem), _dp, _ip, _dp, _dp, _dp, _dp, _dp]
@@ -139,7 +149,8 @@ class PackedProblem:
 
     def __init__(self, eps_cross, coords, freq, mode_spec, symmetry=(0, 0), direction="+", eps_packed=None, basis_fields=None,
                  mu_cross=None, target_override=None, incidence=False, post=0, section=None, grid_correction=None, plane_bounds=None,
-                 eps_dfreq=None, derivatives=False, eps_d2freq=None, second=False, eps_d3freq=None, third=False, left_solve=False):
+                 eps_dfreq=None, derivatives=False, eps_d2freq=None, second=False, eps_d3freq=None, third=False, left_solve=False, eps_d4freq=None,
+                 fourth=False):
         self.section = None
         if section is not None:  # geometric cross-section rasterised on the device (tidy3d_b200/sections.py); no eps array
             self.section, self._section_arrays = section.pack(float(freq), (len(coords[0]) - 1, len(coords[1]) - 1), dispersion=derivatives,
@@ -258,6 +269,19 @@ class PackedProblem:
                 raise ValueError("eps_d3freq must have the nine components and the shape of eps_cross")
             p.eps_d3freq = _ptr(self.eps_d3freq.view(np.float64))
         p.left_solve = 1 if left_solve else 0
+        self.ext = ProblemExt()  # the fourth-order inputs (b200ms_problem_ext)
+        self.eps_d4freq = self.d4eps_table = None
+        if eps_d4freq is not None:  # d^4 eps_cross / df^4 in the eps layout (material term of the fourth derivative)
+            if section is not None:
+                raise ValueError("eps_d4freq belongs to an eps_cross problem; a section's media carry their own dispersion")
+            self.eps_d4freq = np.ascontiguousarray(np.stack([np.asarray(eps_d4freq[i], dtype=np.complex128) for i in range(len(eps_d4freq))]))
+            if self.eps_d4freq.shape != (9, self.nx, self.ny):
+                raise ValueError("eps_d4freq must have the nine components and the shape of eps_cross")
+            self.ext.eps_d4freq = _ptr(self.eps_d4freq.view(np.float64))
+        if fourth and section is not None:
+            self.d4eps_table = section.d4_table(float(freq))
+            if self.d4eps_table is not None:
+                self.ext.d4eps_table = _ptr(self.d4eps_table.view(np.float64))
         self.struct = p
         self.num_modes = p.num_modes
 
@@ -349,7 +373,7 @@ class Handle:
             pass
 
     def solve_batch(self, packed, want_fields=True, fields_ptrs=None, want_flux=False, want_overlaps=False, want_dfreq=False, want_deps=False,
-                    want_d2freq=False, want_group_eps=False, want_d3freq=False, want_deps_tensor=False):
+                    want_d2freq=False, want_group_eps=False, want_d3freq=False, want_deps_tensor=False, want_d4freq=False):
         """packed: list of PackedProblem.  Returns (rc, fields list | None, n_complex list, Result structs).
 
         ``fields_ptrs``: optional list of raw addresses (host or DEVICE memory, e.g. ``tensor.data_ptr()``) the library
@@ -359,15 +383,21 @@ class Handle:
         the residual of its correction solve (``last_d2n_dfreq2`` / ``last_d2n_residual``); ``want_group_eps``: d(dn/df) / d eps of
         every mode from that correction solve (``last_d2n_dfreq_deps``); ``want_d3freq``: d^3 n / df^3 of every mode from the same
         correction solve (``last_d3n_dfreq3``); ``want_deps_tensor``: the nine-component d n / d eps of every mode (result.dn_deps_tensor,
-        (9, nx, ny, M) arrays in ``last_dn_deps``; not together with ``want_deps``)."""
+        (9, nx, ny, M) arrays in ``last_dn_deps``; not together with ``want_deps``); ``want_d4freq``: d^4 n / df^4 of every mode and the
+        residual of its second correction solve (``last_d4n_dfreq4`` / ``last_d4n_residual``, b200ms_solve_batch_ext; needs
+        ``want_d3freq``)."""
         if want_deps and want_deps_tensor:
             raise ValueError("want_deps and want_deps_tensor fill the same list: ask for one of them")
+        if want_d4freq and not want_d3freq:
+            raise ValueError("want_d4freq needs want_d3freq: the fourth derivative is formed from the third-order pass")
         n = len(packed)
         probs = (Problem * n)(*[p.struct for p in packed])
         results = (Result * n)()
         fields, ncs = [], []
         self.last_flux, self.last_te, self.last_overlaps, self.last_dn_dfreq, self.last_dn_deps = [], [], [], [], []
         self.last_d2n_dfreq2, self.last_d2n_residual, self.last_d2n_dfreq_deps, self.last_d3n_dfreq3 = [], [], [], []
+        self.last_d4n_dfreq4, self.last_d4n_residual = [], []
+        rext = (ResultExt * n)() if want_d4freq else None
         for i, p in enumerate(packed):
             nc = np.zeros(p.num_modes, dtype=np.complex128)
             ncs.append(nc)
@@ -398,6 +428,12 @@ class Handle:
                 d = np.zeros(p.num_modes, dtype=np.complex128)
                 self.last_d3n_dfreq3.append(d)
                 results[i].d3n_dfreq3 = _ptr(d.view(np.float64))
+            if want_d4freq:
+                d, r = np.zeros(p.num_modes, dtype=np.complex128), np.zeros(p.num_modes)
+                self.last_d4n_dfreq4.append(d)
+                self.last_d4n_residual.append(r)
+                rext[i].d4n_dfreq4 = _ptr(d.view(np.float64))
+                rext[i].d4n_residual = _ptr(r)
             if want_flux:
                 fl, te = np.zeros(p.num_modes), np.zeros(p.num_modes)
                 self.last_flux.append(fl)
@@ -417,5 +453,9 @@ class Handle:
                 results[i].fields = C.cast(C.c_void_p(f.ctypes.data), _dp)
             else:
                 results[i].fields = None
-        rc = lib().b200ms_solve_batch(self._h, n, probs, results)
+        if want_d4freq:
+            pext = (ProblemExt * n)(*[p.ext for p in packed])
+            rc = lib().b200ms_solve_batch_ext(self._h, n, probs, results, pext, rext)
+        else:
+            rc = lib().b200ms_solve_batch(self._h, n, probs, results)
         return rc, (fields if (want_fields and fields_ptrs is None) else None), ncs, results

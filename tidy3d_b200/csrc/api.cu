@@ -74,6 +74,8 @@ struct b200ms_handle {
   unsigned char *flush_buf = nullptr;
   size_t flush_bytes = 0;
   b200ms_stats stats;
+  const b200ms_problem_ext *pext = nullptr;  // the fourth-order arrays of the b200ms_solve_batch_ext call in progress, or null
+  const b200ms_result_ext *rext = nullptr;
 };
 
 extern "C" int b200ms_version(void) { return B200MS_VERSION; }
@@ -714,7 +716,7 @@ bool batch_refs(const Window &W, const std::vector<int> &ids, std::vector<const 
 }
 
 // The diagonal (xx, yy, zz; ncomp = 3) or all nine components (ncomp = 9) of a per-problem input in the layout of `eps` -- the
-// caller's array `arr(p)`, or for a section the rasteriser fed with the per-medium table `tab(sec)` -- into dst [B][ncomp][N],
+// caller's array `arr(p)`, or for a section the rasteriser fed with the per-medium table `tab(p)` -- into dst [B][ncomp][N],
 // zero where a problem has neither.  `scratch` holds one rasterised section (9 N complex values, then the section upload); the
 // stream is synchronised after every problem.
 template <typename Arr, typename Tab>
@@ -729,10 +731,10 @@ void gather_diag(b200ms_handle *h, const std::vector<int> &ids, const Window &W,
     const cplx *src = nullptr;
     if (p.eps && arr(p)) {
       src = reinterpret_cast<const cplx *>(arr(p));
-    } else if (!p.eps && tab(*p.section)) {  // the medium's rasteriser, fed with the derivative table
+    } else if (!p.eps && tab(p)) {  // the medium's rasteriser, fed with the derivative table
       size_t bytes = 0;
       cplx *full = reinterpret_cast<cplx *>(scratch);
-      SectionDev sd = upload_section(*p.section, p, tab(*p.section), scratch + align256(9 * N * sizeof(cplx)), st, bytes);
+      SectionDev sd = upload_section(*p.section, p, tab(p), scratch + align256(9 * N * sizeof(cplx)), st, bytes);
       section_raster_kernel<<<(unsigned)std::min<size_t>((N + 255) / 256, 2048), 256, 0, st>>>(sd, nx, ny, full);
       CUDA_CHECK(cudaGetLastError());
       src = full;
@@ -753,7 +755,7 @@ size_t gather_scratch_bytes(const std::vector<int> &ids, const Window &W, const 
   size_t bytes = 0;
   for (int id : ids) {
     const b200ms_problem &p = prob[W.i0 + id];
-    if (!p.eps && tab(*p.section))
+    if (!p.eps && tab(p))
       bytes = std::max(bytes, section_device_bytes(*p.section, nx, ny) + align256(9 * (size_t)nx * ny * sizeof(cplx)));
   }
   return bytes;
@@ -804,7 +806,7 @@ void derivative_pass(b200ms_handle *h, BatchSolver<T, C, P, PC> &S, const std::v
   const size_t o_deps = o_scale + align256((size_t)B * k * sizeof(cplx));
   size_t o_map = o_deps + (any_disp ? align256((size_t)B * 3 * N * sizeof(cplx)) : 0);
   auto arr1 = [](const b200ms_problem &p) { return p.eps_dfreq; };
-  auto tab1 = [](const b200ms_section &sec) { return sec.deps_table; };
+  auto tab1 = [](const b200ms_problem &p) { return p.section->deps_table; };
   const size_t sec_bytes = gather_scratch_bytes(ids, W, prob, nx, ny, tab1);
   const size_t o_zero = o_map + (any_map ? align256((size_t)B * 3 * N * k * sizeof(cplx)) : 0);  // zero rows of dn_deps_tensor
   const size_t o_sec = o_zero + (any_map ? align256(N * k * sizeof(cplx)) : 0);
@@ -971,7 +973,7 @@ void tensor_derivative_pass(b200ms_handle *h, BatchSolver<T, C, P, PC> &S, const
     const size_t o_deps = o_scale + align256((size_t)B * k * sizeof(cplx));
     const size_t o_map = o_deps + (any_disp ? align256((size_t)B * 9 * N * sizeof(cplx)) : 0);
     auto arr1 = [](const b200ms_problem &p) { return p.eps_dfreq; };
-    auto tab1 = [](const b200ms_section &sec) { return sec.deps_table; };
+    auto tab1 = [](const b200ms_problem &p) { return p.section->deps_table; };
     const size_t sec_bytes = gather_scratch_bytes(ids, W, prob, nx, ny, tab1);
     const size_t o_sec = o_map + (any_map ? align256((size_t)B * 9 * N * k * sizeof(cplx)) : 0);
     h->deriv.reserve(o_sec + sec_bytes + 256);
@@ -1049,33 +1051,45 @@ void tensor_derivative_pass(b200ms_handle *h, BatchSolver<T, C, P, PC> &S, const
 // r = -Pi A'v, one correction solve (A - lambda_q) x = r by the eigen-solve's own inner solver (Krylov shift lambda_q of every
 // problem; the multigrid stays built for sigma) and a scan for w^T A'x.  With result.d2n_dfreq_deps, group_grad_kernel then
 // sums w_hat^T v and writes slot q of the map from the same x; with result.d3n_dfreq3, third_scan_kernel sums the six
-// products of lambda''' from the same x.  It writes its own buffers, the first two slots of the outer Krylov basis and the
-// inner solver's scratch -- nothing the fields, the post-processing or the warm start read.
+// products of lambda''' from the same x.  With b200ms_result_ext.d4n_dfreq4 (which needs d3n_dfreq3), fourth_rhs_kernel then
+// writes r2 from the same x, a second correction solve (A - lambda_q) x2 = r2 runs at the same shift, and fourth_scan_kernel
+// sums the products of lambda''''.  It writes its own buffers, the first four slots of the outer Krylov basis and the inner
+// solver's scratch -- nothing the fields, the post-processing or the warm start read.
 template <typename T, typename C, typename P, typename PC>
 void dispersion_pass(b200ms_handle *h, BatchSolver<T, C, P, PC> &S, const std::vector<const ProblemSetup *> &ps, const std::vector<int> &ids,
                      const Window &W, const b200ms_problem *prob, b200ms_result *res, const std::vector<cd> &nsorted,
                      const std::vector<cd> &lam, const DerivArgs<T, C> &da) {
   const int B = (int)ids.size(), k = S.k, nx = S.nx, ny = S.ny;
   const size_t N = (size_t)nx * ny;
-  std::vector<char> skip(B);
-  bool any_mat = false, any_gmap = false, any_third = false;
+  std::vector<char> skip(B), skip4(B, 1);
+  bool any_mat = false, any_gmap = false, any_third = false, any_fourth = false;
   for (int b = 0; b < B; ++b) {
     const b200ms_problem &p = prob[W.i0 + ids[b]];
     const b200ms_result &rb = res[W.i0 + ids[b]];
     skip[b] = (rb.d2n_dfreq2 || rb.d2n_dfreq_deps || rb.d3n_dfreq3) ? 0 : 1;
     any_gmap = any_gmap || rb.d2n_dfreq_deps;
     any_third = any_third || rb.d3n_dfreq3;
+    skip4[b] = (h->rext && h->rext[W.i0 + ids[b]].d4n_dfreq4) ? 0 : 1;
+    any_fourth = any_fourth || !skip4[b];
     any_mat = any_mat || (p.eps ? (p.eps_dfreq || p.eps_d2freq) : (p.section->deps_table || p.section->d2eps_table));
   }
   for (int b = 0; b < B && any_third; ++b) {  // the third-order terms also read eps'''
     const b200ms_problem &p = prob[W.i0 + ids[b]];
     any_mat = any_mat || (p.eps ? p.eps_d3freq != nullptr : p.section->d3eps_table != nullptr);
   }
+  for (int b = 0; b < B && any_fourth; ++b) {  // and the fourth-order terms eps''''
+    const b200ms_problem &p = prob[W.i0 + ids[b]];
+    const b200ms_problem_ext *e = h->pext ? h->pext + W.i0 + ids[b] : nullptr;
+    any_mat = any_mat || (e && (p.eps ? e->eps_d4freq != nullptr : e->d4eps_table != nullptr));
+  }
   // host tables: f^2 d^2c/df^2 = 2 (f dc/df)^2 / c = 2 c (kappa / s)^2, frequencies; for the third-order pass
-  // f^3 d^3c/df^3 = -6 c (kappa / s)^3 and the combined directions c' +- c''
+  // f^3 d^3c/df^3 = -6 c (kappa / s)^3 and the combined directions c' +- c''; for the fourth-order pass
+  // f^4 d^4c/df^4 = 24 c (kappa / s)^4 and c' +- c'''
   std::vector<T> c2x((size_t)B * 4 * nx), c2y((size_t)B * 4 * ny);
   const size_t n3x = any_third ? (size_t)B * 4 * nx : 0, n3y = any_third ? (size_t)B * 4 * ny : 0;
   std::vector<T> c3x(n3x), c3y(n3y), csx(n3x), csy(n3y), cdx(n3x), cdy(n3y);
+  const size_t n4x = any_fourth ? n3x : 0, n4y = any_fourth ? n3y : 0;
+  std::vector<T> c4x(n4x), c4y(n4y), qsx(n4x), qsy(n4y), qdx(n4x), qdy(n4y);
   std::vector<double> freq(B);
   for (int b = 0; b < B; ++b) {
     freq[b] = prob[W.i0 + ids[b]].freq;
@@ -1102,16 +1116,25 @@ void dispersion_pass(b200ms_handle *h, BatchSolver<T, C, P, PC> &S, const std::v
           (a == 0 ? c3x : c3y)[o + (size_t)w * n + i] = from_cd<T>(-6.0 * cw * r * r * r);
           (a == 0 ? csx : csy)[o + (size_t)w * n + i] = from_cd<T>(d1 + d2);
           (a == 0 ? cdx : cdy)[o + (size_t)w * n + i] = from_cd<T>(d1 - d2);
+          if (!any_fourth) continue;
+          const cd d3 = -6.0 * cw * r * r * r;
+          (a == 0 ? c4x : c4y)[o + (size_t)w * n + i] = from_cd<T>(24.0 * cw * (r * r) * (r * r));
+          (a == 0 ? qsx : qsy)[o + (size_t)w * n + i] = from_cd<T>(d1 + d3);
+          (a == 0 ? qdx : qdy)[o + (size_t)w * n + i] = from_cd<T>(d1 - d3);
         }
       }
     }
   }
   auto arr1 = [](const b200ms_problem &p) { return p.eps_dfreq; };
-  auto tab1 = [](const b200ms_section &sec) { return sec.deps_table; };
+  auto tab1 = [](const b200ms_problem &p) { return p.section->deps_table; };
   auto arr2 = [](const b200ms_problem &p) { return p.eps_d2freq; };
-  auto tab2 = [](const b200ms_section &sec) { return sec.d2eps_table; };
+  auto tab2 = [](const b200ms_problem &p) { return p.section->d2eps_table; };
   auto arr3 = [](const b200ms_problem &p) { return p.eps_d3freq; };
-  auto tab3 = [](const b200ms_section &sec) { return sec.d3eps_table; };
+  auto tab3 = [](const b200ms_problem &p) { return p.section->d3eps_table; };
+  // the fourth-order inputs live in the b200ms_problem_ext entry of the same index
+  const b200ms_problem_ext *pext = h->pext;
+  auto arr4 = [pext, prob](const b200ms_problem &p) { return pext ? pext[&p - prob].eps_d4freq : nullptr; };
+  auto tab4 = [pext, prob](const b200ms_problem &p) { return pext ? pext[&p - prob].d4eps_table : nullptr; };
   const int nch = (int)std::min<size_t>(kDerivChunks, (N + 255) / 256);
   const size_t o_c2x = 0, o_c2y = align256(c2x.size() * sizeof(T)), o_f = o_c2y + align256(c2y.size() * sizeof(T));
   const size_t o_part = o_f + align256(B * sizeof(double)), o_sum = o_part + align256((size_t)B * nch * 3 * sizeof(cplx));
@@ -1119,6 +1142,7 @@ void dispersion_pass(b200ms_handle *h, BatchSolver<T, C, P, PC> &S, const std::v
   const size_t pbytes = any_mat ? align256((size_t)B * 3 * N * sizeof(cplx)) : 0, o_p2 = o_p1 + pbytes, o_sec = o_p2 + pbytes;
   size_t sec_bytes = any_mat ? std::max(gather_scratch_bytes(ids, W, prob, nx, ny, tab1), gather_scratch_bytes(ids, W, prob, nx, ny, tab2)) : 0;
   if (any_mat && any_third) sec_bytes = std::max(sec_bytes, gather_scratch_bytes(ids, W, prob, nx, ny, tab3));
+  if (any_mat && any_fourth) sec_bytes = std::max(sec_bytes, gather_scratch_bytes(ids, W, prob, nx, ny, tab4));
   // group-gradient pass: per-problem (alpha, beta), the sum w_hat^T v and the map [B][3][N][M]
   const size_t o_ab = align256(o_sec + sec_bytes), o_hsum = o_ab + align256((size_t)B * 2 * sizeof(cplx));
   const size_t o_gmap = o_hsum + align256((size_t)B * 3 * sizeof(cplx));
@@ -1137,6 +1161,23 @@ void dispersion_pass(b200ms_handle *h, BatchSolver<T, C, P, PC> &S, const std::v
     o_tsum = end;
     end += align256((size_t)B * 6 * sizeof(cplx));
   }
+  // fourth-order pass: c'''', c' + c''', c' - c''' per axis, p'''', p' + p''', p' - p''', (lambda', lambda'', lambda) per problem,
+  // its partial sums [B][4][nch][3] and the twelve sums per problem
+  size_t o_c4[6] = {0, 0, 0, 0, 0, 0}, o_p4 = 0, o_sc = 0, o_fpart = 0, o_fsum = 0;
+  if (any_fourth) {
+    for (int e = 0; e < 6; ++e) {
+      o_c4[e] = end;
+      end += align256((e % 2 == 0 ? n4x : n4y) * sizeof(T));
+    }
+    o_p4 = end;
+    end += 3 * pbytes;
+    o_sc = end;
+    end += align256((size_t)B * 3 * sizeof(cplx));
+    o_fpart = end;
+    end += align256((size_t)B * 4 * nch * 3 * sizeof(cplx));
+    o_fsum = end;
+    end += align256((size_t)B * 12 * sizeof(cplx));
+  }
   h->disp.reserve(end + 256);
   unsigned char *base = h->disp.p;
   cudaStream_t st = h->stream;
@@ -1152,16 +1193,22 @@ void dispersion_pass(b200ms_handle *h, BatchSolver<T, C, P, PC> &S, const std::v
     cplx *p1 = reinterpret_cast<cplx *>(base + o_p1), *p2 = reinterpret_cast<cplx *>(base + o_p2);
     gather_diag(h, ids, W, prob, nx, ny, arr1, tab1, p1, base + o_sec);
     gather_diag(h, ids, W, prob, nx, ny, arr2, tab2, p2, base + o_sec);
-    cplx *p3 = nullptr, *pps = nullptr, *ppd = nullptr;
+    cplx *p3 = nullptr, *pps = nullptr, *ppd = nullptr, *p4 = nullptr, *pqs = nullptr, *pqd = nullptr;
     if (any_third) {
       p3 = reinterpret_cast<cplx *>(base + o_p3);
       pps = reinterpret_cast<cplx *>(base + o_p3 + pbytes);
       ppd = reinterpret_cast<cplx *>(base + o_p3 + 2 * pbytes);
       gather_diag(h, ids, W, prob, nx, ny, arr3, tab3, p3, base + o_sec);
     }
+    if (any_fourth) {
+      p4 = reinterpret_cast<cplx *>(base + o_p4);
+      pqs = reinterpret_cast<cplx *>(base + o_p4 + pbytes);
+      pqd = reinterpret_cast<cplx *>(base + o_p4 + 2 * pbytes);
+      gather_diag(h, ids, W, prob, nx, ny, arr4, tab4, p4, base + o_sec);
+    }
     disp_fields_kernel<C><<<(unsigned)std::min<size_t>(((size_t)B * N + 255) / 256, 4096), 256, 0, st>>>(
         nx, ny, B, da.fields, da.field_bstride, da.jz_e, da.jz_axis, da.jz_len, reinterpret_cast<const double *>(base + o_f), p1, p2, p3,
-        pps, ppd);
+        pps, ppd, p4, pqs, pqd);
     CUDA_CHECK(cudaGetLastError());
     h->stats.launches += 1;
     a.p1 = p1;
@@ -1188,6 +1235,26 @@ void dispersion_pass(b200ms_handle *h, BatchSolver<T, C, P, PC> &S, const std::v
     }
     ta.partial = reinterpret_cast<cplx *>(base + o_tpart);
   }
+  FourthArgs<T> fa{};
+  cplx *dsc = nullptr, *fsum = nullptr;
+  if (any_fourth) {
+    const std::vector<T> *tabs[6] = {&c4x, &c4y, &qsx, &qsy, &qdx, &qdy};
+    for (int e = 0; e < 6; ++e)
+      CUDA_CHECK(cudaMemcpyAsync(base + o_c4[e], tabs[e]->data(), tabs[e]->size() * sizeof(T), cudaMemcpyHostToDevice, st));
+    fa.c4x = reinterpret_cast<const T *>(base + o_c4[0]); fa.c4y = reinterpret_cast<const T *>(base + o_c4[1]);
+    fa.qsx = reinterpret_cast<const T *>(base + o_c4[2]); fa.qsy = reinterpret_cast<const T *>(base + o_c4[3]);
+    fa.qdx = reinterpret_cast<const T *>(base + o_c4[4]); fa.qdy = reinterpret_cast<const T *>(base + o_c4[5]);
+    if (a.p1) {
+      fa.p4 = reinterpret_cast<const cplx *>(base + o_p4);
+      fa.qs = reinterpret_cast<const cplx *>(base + o_p4 + pbytes);
+      fa.qd = reinterpret_cast<const cplx *>(base + o_p4 + 2 * pbytes);
+    }
+    dsc = reinterpret_cast<cplx *>(base + o_sc);
+    fsum = reinterpret_cast<cplx *>(base + o_fsum);
+    fa.sc = dsc;
+    fa.x2 = S.basis0() + 3 * S.vstride;  // r2 in slot 2, x2 in slot 3
+    fa.partial = reinterpret_cast<cplx *>(base + o_fpart);
+  }
   auto scan = [&](int phase, std::vector<cplx> &sums) {
     const dim3 g(phase == 1 ? (unsigned)std::min<size_t>((N + 255) / 256, 1024) : (unsigned)nch, B);
     if (S.has_mu) disp_scan_kernel<T, C, true><<<g, 256, 0, st>>>(a, phase);
@@ -1206,6 +1273,7 @@ void dispersion_pass(b200ms_handle *h, BatchSolver<T, C, P, PC> &S, const std::v
   for (int q = 0; q < k; ++q) {
     a.q = q;
     std::vector<cplx> sv, sx;
+    std::vector<cd> l3v(B);  // f^3 d^3 lambda / df^3 of the third-order pass, for the fourth-order one
     scan(0, sv);  // w^T v, w^T A'v, w^T A''v
     std::vector<cplx> beta(B);
     std::vector<cd> shift(B);
@@ -1289,6 +1357,7 @@ void dispersion_pass(b200ms_handle *h, BatchSolver<T, C, P, PC> &S, const std::v
         const cd l2 = (zc(s[2]) + 2.0 * (zc(t[1]) - l1 * wx)) / wv;
         const cd hv = zc(u[0]), hx = zc(u[1]), w3v = zc(u[2]), h2v = zc(u[3]), w2x = zc(u[4]), h1x = zc(u[5]);
         const cd l3 = (w3v + 3.0 * h2v + 3.0 * w2x + 6.0 * h1x - 6.0 * l1 * hx - 3.0 * l2 * (hv + wx)) / wv;  // f^3 d^3 lambda / df^3
+        l3v[b] = l3;
         const double f = freq[b];
         const cd dl = l1 / f, d2l = l2 / (f * f), d3l = l3 / (f * f * f);
         const cd sn = nsorted[(size_t)b * k + q];
@@ -1297,6 +1366,64 @@ void dispersion_pass(b200ms_handle *h, BatchSolver<T, C, P, PC> &S, const std::v
         if (std::abs(wv) == 0 || !(resv[b] <= 100.0 * tol)) d3n = cd(std::nan(""), std::nan(""));
         rr.d3n_dfreq3[2 * q] = d3n.real();
         rr.d3n_dfreq3[2 * q + 1] = d3n.imag();
+      }
+    }
+    if (any_fourth) {  // lambda'''' of slot q: r2 from the same x, the second correction solve, then the two scans
+      auto zc = [](const cplx &z) { return cd(z.re, z.im); };
+      std::vector<cplx> sc((size_t)B * 3);
+      for (int b = 0; b < B; ++b) {
+        const cplx *s = sv.data() + (size_t)b * 3, *t = sx.data() + (size_t)b * 3;
+        const cd wv = zc(s[0]), l1 = std::abs(wv) > 0 ? zc(s[1]) / wv : cd(0, 0);
+        const cd l2 = std::abs(wv) > 0 ? (zc(s[2]) + 2.0 * (zc(t[1]) - l1 * zc(t[0]))) / wv : cd(0, 0);
+        const cd lq = lam[(size_t)b * k + q];
+        sc[3 * b] = mk(l1.real(), l1.imag());
+        sc[3 * b + 1] = mk(l2.real(), l2.imag());
+        sc[3 * b + 2] = mk(lq.real(), lq.imag());
+      }
+      CUDA_CHECK(cudaMemcpyAsync(dsc, sc.data(), sc.size() * sizeof(cplx), cudaMemcpyHostToDevice, st));
+      T *r2 = S.basis0() + 2 * S.vstride, *x2 = S.basis0() + 3 * S.vstride;
+      const dim3 g1((unsigned)std::min<size_t>((N + 255) / 256, 1024), B), g0(nch, B);
+      if (S.has_mu) fourth_rhs_kernel<T, C, true><<<g1, 256, 0, st>>>(a, dsc, r2);
+      else fourth_rhs_kernel<T, C, false><<<g1, 256, 0, st>>>(a, dsc, r2);
+      CUDA_CHECK(cudaGetLastError());
+      h->stats.launches += 1;
+      int iters2 = 0;
+      std::vector<double> resv2;
+      S.solve_op(r2, x2, iters2, &skip4, nullptr, &resv2);
+      if (S.has_mu) {
+        fourth_scan_kernel<T, C, true, 0><<<g0, 256, 0, st>>>(a, ta, fa);
+        fourth_scan_kernel<T, C, true, 1><<<g0, 256, 0, st>>>(a, ta, fa);
+      } else {
+        fourth_scan_kernel<T, C, false, 0><<<g0, 256, 0, st>>>(a, ta, fa);
+        fourth_scan_kernel<T, C, false, 1><<<g0, 256, 0, st>>>(a, ta, fa);
+      }
+      deriv_final_kernel<<<(B * 12 + 127) / 128, 128, 0, st>>>(fa.partial, nch, B * 12, fsum);
+      CUDA_CHECK(cudaGetLastError());
+      h->stats.launches += 3;
+      std::vector<cplx> s4((size_t)B * 12), s3((size_t)B * 6);
+      CUDA_CHECK(cudaMemcpyAsync(s4.data(), fsum, s4.size() * sizeof(cplx), cudaMemcpyDeviceToHost, st));
+      CUDA_CHECK(cudaMemcpyAsync(s3.data(), reinterpret_cast<cplx *>(base + o_tsum), s3.size() * sizeof(cplx), cudaMemcpyDeviceToHost, st));
+      CUDA_CHECK(cudaStreamSynchronize(st));
+      for (int b = 0; b < B; ++b) {
+        if (skip4[b]) continue;
+        const b200ms_result_ext &re = h->rext[W.i0 + ids[b]];
+        const cplx *s = sv.data() + (size_t)b * 3, *t = sx.data() + (size_t)b * 3, *u = s3.data() + (size_t)b * 6, *z = s4.data() + (size_t)b * 12;
+        const cd wv = zc(s[0]), l1 = zc(sc[3 * b]), l2 = zc(sc[3 * b + 1]), l3 = l3v[b];
+        // z: w^T (A''''v + 4 A'''x), w_hat^T A'''v, 0 | w_hat2^T (12 A''v + 24 A'x + 24 (A - lambda) x2), w^T A''x2, w_hat^T (12 A''x +
+        // 24 A'x2), w_hat2^T v, w^T x2, w_hat2^T x, w_hat^T x2, 0, 0
+        const cd num = zc(z[0]) + 4.0 * zc(z[1]) + zc(z[3]) + 12.0 * zc(z[4]) + zc(z[5]);
+        const cd D1 = zc(u[0]) + zc(t[0]), D2 = zc(z[6]) + zc(u[1]) + zc(z[7]), D3 = zc(z[8]) + zc(z[9]);
+        const cd l4 = (num - 24.0 * l1 * D3 - 12.0 * l2 * D2 - 4.0 * l3 * D1) / wv;  // f^4 d^4 lambda / df^4
+        const double f = freq[b];
+        const cd dl = l1 / f, d2l = l2 / (f * f), d3l = l3 / (f * f * f), d4l = l4 / ((f * f) * (f * f));
+        const cd sn = nsorted[(size_t)b * k + q];
+        const cd ds = -dl / (2.0 * sn), d2s = -(d2l + 2.0 * ds * ds) / (2.0 * sn), d3s = -(d3l + 6.0 * ds * d2s) / (2.0 * sn);
+        const cd d4s = -(d4l + 8.0 * ds * d3s + 6.0 * d2s * d2s) / (2.0 * sn);
+        cd d4n = ps[b]->knorm * d4s;
+        if (std::abs(wv) == 0 || !(resv[b] <= 100.0 * tol) || !(resv2[b] <= 100.0 * tol)) d4n = cd(std::nan(""), std::nan(""));
+        re.d4n_dfreq4[2 * q] = d4n.real();
+        re.d4n_dfreq4[2 * q + 1] = d4n.imag();
+        if (re.d4n_residual) re.d4n_residual[q] = resv2[b];
       }
     }
   }
@@ -1513,8 +1640,8 @@ void dispatch_group(int kind, bool f32, A &&...a) {
 
 }  // namespace
 
-extern "C" int b200ms_solve_batch(b200ms_handle *h, int nprob, const b200ms_problem *prob, b200ms_result *res) {
-  if (!h || nprob < 0 || (nprob > 0 && (!prob || !res))) return B200MS_ERR_ARG;
+// The solve itself (b200ms_solve_batch_ext after its own checks; the fourth-order arrays are in h->pext / h->rext).
+static int solve_batch_impl(b200ms_handle *h, int nprob, const b200ms_problem *prob, b200ms_result *res) {
   if (cudaSetDevice(h->device) != cudaSuccess) return B200MS_ERR_CUDA;
   h->err.clear();
   std::memset(&h->stats, 0, sizeof(h->stats));
@@ -1670,6 +1797,33 @@ extern "C" int b200ms_solve_batch(b200ms_handle *h, int nprob, const b200ms_prob
   }
   h->stats.total_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - call0).count();
   return first_err;
+}
+
+extern "C" int b200ms_solve_batch_ext(b200ms_handle *h, int nprob, const b200ms_problem *prob, b200ms_result *res,
+                                      const b200ms_problem_ext *pext, const b200ms_result_ext *rext) {
+  if (!h || nprob < 0 || (nprob > 0 && (!prob || !res))) return B200MS_ERR_ARG;
+  for (int i = 0; i < nprob && rext; ++i) {
+    if (rext[i].d4n_dfreq4 && !res[i].d3n_dfreq3) {  // lambda'''' is formed from the third-order pass of the same slot
+      h->err = "d4n_dfreq4 needs d3n_dfreq3 of the same problem";
+      res[i].status = B200MS_ERR_ARG;
+      return B200MS_ERR_ARG;
+    }
+    if (pext && pext[i].eps_d4freq && !prob[i].eps) {
+      h->err = "eps_d4freq belongs to an eps problem; a section's media carry d4eps_table";
+      res[i].status = B200MS_ERR_ARG;
+      return B200MS_ERR_ARG;
+    }
+  }
+  h->pext = pext;
+  h->rext = rext;
+  const int rc = solve_batch_impl(h, nprob, prob, res);
+  h->pext = nullptr;
+  h->rext = nullptr;
+  return rc;
+}
+
+extern "C" int b200ms_solve_batch(b200ms_handle *h, int nprob, const b200ms_problem *prob, b200ms_result *res) {
+  return b200ms_solve_batch_ext(h, nprob, prob, res, nullptr, nullptr);
 }
 
 // ---- benchmark hook -----------------------------------------------------------------------------------

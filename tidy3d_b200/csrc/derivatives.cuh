@@ -316,10 +316,13 @@ __global__ void __launch_bounds__(256) disp_scan_kernel(DispArgs<T, C> a, int ph
 // diagonal (in place: dp1 holds d eps / df on entry, dp2 d^2 eps / df^2).  Bend: exx = eps_xx / je, eyy = eps_yy / je,
 // ezz = je eps_zz; freq: [B] Hz.  iez' = -ezz' iez^2, iez'' = 2 ezz'^2 iez^3 - ezz'' iez^2.  PEC-valued cells: 0 (as eps_grad).
 // With dp3 (the third-order pass): dp3 holds d^3 eps / df^3 on entry and receives f^3 d^3p/df^3, iez''' = -ezz''' iez^2 +
-// 6 ezz' ezz'' iez^3 - 6 ezz'^3 iez^4, and dps / dpd receive the combined directions p' + p'' and p' - p''.
+// 6 ezz' ezz'' iez^3 - 6 ezz'^3 iez^4, and dps / dpd receive the combined directions p' + p'' and p' - p''.  With dp4 as well (the
+// fourth-order pass): dp4 holds d^4 eps / df^4 on entry and receives f^4 d^4p/df^4, iez'''' = -ezz'''' iez^2 + (8 ezz' ezz''' +
+// 6 ezz''^2) iez^3 - 36 ezz'^2 ezz'' iez^4 + 24 ezz'^4 iez^5, and dqs / dqd receive p' + p''' and p' - p'''.
 template <typename C>
 __global__ void disp_fields_kernel(int nx, int ny, int B, const C *fields, size_t field_bstride, const double *jz_e, int jz_axis, int jz_len,
-                                   const double *freq, cplx *dp1, cplx *dp2, cplx *dp3, cplx *dps, cplx *dpd) {
+                                   const double *freq, cplx *dp1, cplx *dp2, cplx *dp3, cplx *dps, cplx *dpd, cplx *dp4, cplx *dqs,
+                                   cplx *dqd) {
   const size_t N = (size_t)nx * ny;
   for (size_t t = (size_t)blockIdx.x * blockDim.x + threadIdx.x; t < (size_t)B * N; t += (size_t)gridDim.x * blockDim.x) {
     const int b = (int)(t / N);
@@ -352,6 +355,21 @@ __global__ void disp_fields_kernel(int nx, int ny, int B, const C *fields, size_
     for (int k = 0; k < 3; ++k) {
       ds[(size_t)k * N] = d1[(size_t)k * N] + d2[(size_t)k * N];
       dd[(size_t)k * N] = d1[(size_t)k * N] - d2[(size_t)k * N];
+    }
+    if (!dp4) continue;
+    cplx *d4 = dp4 + (size_t)b * 3 * N + g, *qs = dqs + (size_t)b * 3 * N + g, *qd = dqd + (size_t)b * 3 * N + g;
+    const double f4 = (f * f) * (f * f);
+    for (int k = 0; k < 2; ++k) {
+      const bool pk = abs2(to_cplx(ldg(fb + (size_t)k * N + g))) >= pec * pec;
+      d4[(size_t)k * N] = pk ? mk(0.0, 0.0) : d4[(size_t)k * N] * (f4 / je);
+    }
+    const cplx e4 = d4[2 * N] * (f4 * je);  // f^4 ezz''''
+    const cplx iz3 = iz2 * iz, iz4 = iz2 * iz2;
+    d4[2 * N] = is_pec ? mk(0.0, 0.0)
+                       : (8.0 * (e1 * e3) + 6.0 * (e2 * e2)) * iz3 - e4 * iz2 - 36.0 * (e1 * e1 * e2) * iz4 + 24.0 * ((e1 * e1) * (e1 * e1)) * (iz4 * iz);
+    for (int k = 0; k < 3; ++k) {
+      qs[(size_t)k * N] = d1[(size_t)k * N] + d3[(size_t)k * N];
+      qd[(size_t)k * N] = d1[(size_t)k * N] - d3[(size_t)k * N];
     }
   }
 }
@@ -668,6 +686,313 @@ __global__ void __launch_bounds__(256) third_scan_kernel(DispArgs<T, C> a, Third
     __syncthreads();
   }
   if (threadIdx.x < 6) t.partial[(((size_t)b * 2 + threadIdx.x / 3) * gridDim.x + blockIdx.x) * 3 + threadIdx.x % 3] = red[threadIdx.x][0];
+}
+
+// ------------------------------------------------------------------------------------------------
+// Fourth-order pass: the fourth frequency derivative of lambda from a second-order right correction x2 and the structural
+// second-order left correction w_hat2 (oracle/mode_fourth_order.py is the float64 model).  Per mode slot, after every stage of
+// the slot that reads x: fourth_rhs_kernel writes r2 = -[(A' - lambda') x + (A'' - lambda'') v / 2] (w^T r2 = 0 is the formula
+// for lambda''), the eigen-solve's inner solver gives (A - lambda) x2 = r2, and fourth_scan_kernel sums (PART 0)
+//   w^T (A''''v + 4 A'''x),  w_hat^T A'''v
+// and (PART 1)
+//   w_hat2^T (12 A''v + 24 A'x + 24 (A - lambda) x2),  w^T A''x2,  w_hat^T (12 A''x + 24 A'x2),  w_hat2^T v,  w^T x2,  w_hat2^T x,
+//   w_hat^T x2,
+// from which the host forms
+//   lambda'''' w^T v = [the five products] - 24 lambda' D_3 - 12 lambda'' D_2 - 4 lambda''' D_1
+// (D_k: the t^k coefficient of (w + t w_hat + t^2 w_hat2)^T (v + t x + t^2 x2)).  A''''v is exact from the 64 unit-step
+// evaluations of kFourthTerms (the first nine move only the coefficients; their derivation is in fourth_operator of the model).
+// w_hat2 = G_2 J Q v + G_1 J (Q_1 v + Q x) + G J (Q_2 v + Q_1 x + Q x2) is formed per cell like w_hat (SecondCell::ww2).
+// ------------------------------------------------------------------------------------------------
+
+// one operator evaluation of A''''v, in the direction numbering of ThirdTerm extended by 6 c'''' (p''''), 7 c' + c''' (p' + p''')
+// and 8 c' - c''' (p' - p''')
+__constant__ ThirdTerm kFourthTerms[64] = {
+    {6, 0, 1.0, 0.0, 0.5}, {6, 0, -1.0, 0.0, -0.5}, {7, 0, 1.0, 0.0, 1}, {8, 0, 1.0, 0.0, -1}, {8, 0, -1.0, 0.0, -1},
+    {7, 0, -1.0, 0.0, 1}, {2, 0, 1.0, 0.0, 3}, {2, 0, -1.0, 0.0, 3}, {0, 0, 0.0, 0.0, -6}, {2, 0, 1.0, 0.0, -6},
+    {2, 0, -1.0, 0.0, 6}, {0, 0, 0.0, 0.0, 18}, {0, 6, 0.0, 1.0, 0.5}, {0, 6, 0.0, -1.0, -0.5}, {0, 7, 0.0, 1.0, 1},
+    {0, 8, 0.0, 1.0, -1}, {0, 8, 0.0, -1.0, -1}, {0, 7, 0.0, -1.0, 1}, {0, 2, 0.0, 1.0, -3}, {0, 2, 0.0, -1.0, 9},
+    {1, 3, 1.0, 1.0, 1}, {1, 3, 1.0, -1.0, -1}, {1, 3, -1.0, 1.0, -1}, {1, 3, -1.0, -1.0, 1}, {2, 2, 1.0, 1.0, 1.5},
+    {2, 2, 1.0, -1.0, -1.5}, {2, 2, -1.0, 1.0, -1.5}, {2, 2, -1.0, -1.0, 1.5}, {3, 1, 1.0, 1.0, 1}, {3, 1, 1.0, -1.0, -1},
+    {3, 1, -1.0, 1.0, -1}, {3, 1, -1.0, -1.0, 1}, {1, 2, 1.0, 1.0, 3}, {1, 2, 1.0, -1.0, -3}, {1, 2, -1.0, 1.0, 3},
+    {1, 2, -1.0, -1.0, -3}, {4, 1, 1.0, 1.0, 1.5}, {4, 1, 1.0, -1.0, -1.5}, {4, 1, -1.0, 1.0, 1.5}, {4, 1, -1.0, -1.0, -1.5},
+    {5, 1, 1.0, 1.0, -1.5}, {5, 1, 1.0, -1.0, 1.5}, {5, 1, -1.0, 1.0, -1.5}, {5, 1, -1.0, -1.0, 1.5}, {2, 1, 1.0, 1.0, 3},
+    {2, 1, 1.0, -1.0, 3}, {2, 1, -1.0, 1.0, -3}, {2, 1, -1.0, -1.0, -3}, {1, 4, 1.0, 1.0, 1.5}, {1, 4, 1.0, -1.0, 1.5},
+    {1, 4, -1.0, 1.0, -1.5}, {1, 4, -1.0, -1.0, -1.5}, {1, 5, 1.0, 1.0, -1.5}, {1, 5, 1.0, -1.0, -1.5}, {1, 5, -1.0, 1.0, 1.5},
+    {1, 5, -1.0, -1.0, 1.5}, {1, 1, 1.0, 1.0, 6}, {1, 1, 1.0, -1.0, 6}, {1, 1, -1.0, 1.0, 6}, {1, 1, -1.0, -1.0, 6},
+    {1, 0, 1.0, 0.0, -12}, {1, 0, -1.0, 0.0, -12}, {0, 1, 0.0, 1.0, -12}, {0, 1, 0.0, -1.0, -12}};
+
+template <typename T>
+struct FourthArgs {
+  const T *c4x, *c4y;          // [B][4][n] f^4 d^4c/df^4 = 24 c'^4 / c^3
+  const T *qsx, *qsy;          // [B][4][n] c' + c'''
+  const T *qdx, *qdy;          // [B][4][n] c' - c'''
+  const cplx *p4, *qs, *qd;    // [B][3][N] p'''', p' + p''', p' - p''' (null with a nondispersive batch)
+  const T *x2;                 // the second-order correction, batched-vector layout
+  const cplx *sc;              // [B][3] lambda', lambda'', lambda (scaled)
+  cplx *partial;               // [B][4][nchunk][3]
+};
+
+// grid (min(N/256, 1024), B), 256 threads: r2 of mode slot a.q into `r2` while a.x holds its first-order correction
+template <typename T, typename C, bool HAS_MU>
+__global__ void __launch_bounds__(256) fourth_rhs_kernel(DispArgs<T, C> a, const cplx *sc, T *r2) {
+  const int b = blockIdx.y, nx = a.d.nx, ny = a.d.ny;
+  const size_t N = (size_t)nx * ny;
+  const bool hp = a.p1 != nullptr;
+  const DispTerm *tab = hp ? kDispTermsP : kDispTermsC;
+  const int nterm = hp ? 13 : 5;
+  const T *vb = a.d.vec + (size_t)a.q * a.d.vstride + (size_t)b * 2 * N, *xb = a.x + (size_t)b * 2 * N;
+  const T *cxb = a.d.cx + (size_t)b * 4 * nx, *cyb = a.d.cy + (size_t)b * 4 * ny;
+  const T *d1x = a.d.dcx + (size_t)b * 4 * nx, *d1y = a.d.dcy + (size_t)b * 4 * ny;
+  const T *d2x = a.c2x + (size_t)b * 4 * nx, *d2y = a.c2y + (size_t)b * 4 * ny;
+  const cplx *p1 = hp ? a.p1 + (size_t)b * 3 * N : nullptr, *p2 = hp ? a.p2 + (size_t)b * 3 * N : nullptr;
+  const C *fb = a.d.fields + a.d.field_bstride * b;
+  const cplx l1 = sc[3 * b], l2 = sc[3 * b + 1];
+  T *rb = r2 + (size_t)b * 2 * N;
+  for (size_t g = (size_t)blockIdx.x * 256 + threadIdx.x; g < N; g += (size_t)gridDim.x * 256) {
+    const int i = (int)(g / ny), j = (int)(g % ny);
+    cplx y[2] = {mk(0.0, 0.0), mk(0.0, 0.0)};  // (A' - lambda') x + (A'' - lambda'') v / 2, without the lambda terms
+#pragma unroll 1
+    for (int t = 0; t < nterm; ++t) {
+      const DispTerm tm = tab[t];
+      const T *dcx = tm.cdir == 1 ? d1x : (tm.cdir == 2 ? d2x : nullptr), *dcy = tm.cdir == 1 ? d1y : (tm.cdir == 2 ? d2y : nullptr);
+      const cplx *dp = tm.pdir == 1 ? p1 : (tm.pdir == 2 ? p2 : nullptr);
+      const CoefRows<T> CX{cxb, dcx, tm.sc, nx}, CY{cyb, dcy, tm.sc, ny};
+      const PertSite<T, C, HAS_MU> Pv{vb, vb + N, fb, dp, tm.sp, CX, CY, nx, ny, N}, Px{xb, xb + N, fb, dp, tm.sp, CX, CY, nx, ny, N};
+      cplx y1, y2;
+      Pv.apply(i, j, y1, y2);
+      y[0] += (0.5 * tm.w2) * y1;
+      y[1] += (0.5 * tm.w2) * y2;
+      Px.apply(i, j, y1, y2);
+      y[0] += tm.w1 * y1;
+      y[1] += tm.w1 * y2;
+    }
+    for (int c = 0; c < 2; ++c) {
+      const cplx e = to_cplx(ldg(vb + (size_t)c * N + g)), x = to_cplx(ldg(xb + (size_t)c * N + g));
+      rb[(size_t)c * N + g] = cast_to<T>(-(y[c] - l1 * x - (0.5 * l2) * e));
+    }
+  }
+}
+
+// w, w_hat and w_hat2 of one mode slot at a cell: GroupCell (v, x, c', p') with x2, c'' and p''
+template <typename T, typename C, bool HAS_MU>
+struct SecondCell {
+  GroupCell<T, C, HAS_MU> G;
+  const T *x2;
+  const T *c2x, *c2y;  // [4][n] f^2 d^2c/df^2 of this problem
+  const cplx *p2;      // [3][N] f^2 d^2p/df^2, or null
+  // t = imz (Dxf e2 - Dyf e1) at (ii, jj) with the 1-D coefficient rows ax, ay (zero outside the grid)
+  __device__ __forceinline__ cplx t(const T *e, int ii, int jj, const T *ax, const T *ay) const {
+    if (!G.in(ii, jj)) return mk(0.0, 0.0);
+    const int nx = G.nx, ny = G.ny;
+    const size_t N = G.N;
+    return G.imz(ii, jj) * (G.co(ax, nx, 0, ii) * G.ld(e + N, ii, jj) + G.co(ax, nx, 1, ii) * G.ld(e + N, ii + 1, jj) -
+                            G.co(ay, ny, 0, jj) * G.ld(e, ii, jj) - G.co(ay, ny, 1, jj) * G.ld(e, ii, jj + 1));
+  }
+  // (q1, q2) of Q e at (ii, jj): backward rows bx, by applied to the t of the forward rows fx, fy, plus the eps term of `fld`
+  // (k-th field of a [3][N] direction, or the coefficient fields for fld == null) scaled by s
+  __device__ __forceinline__ void q(const T *e, int ii, int jj, const T *bx, const T *by, const T *fx, const T *fy, const cplx *fld,
+                                    double s, cplx &q1, cplx &q2) const {
+    const int nx = G.nx, ny = G.ny;
+    const size_t g = (size_t)ii * ny + jj;
+    q1 = mk(0.0, 0.0);
+    q2 = mk(0.0, 0.0);
+    if (bx) {
+      const cplx t0 = t(e, ii, jj, fx, fy);
+      q1 = G.co(bx, nx, 2, ii) * t0 + G.co(bx, nx, 3, ii) * t(e, ii - 1, jj, fx, fy);
+      q2 = G.co(by, ny, 2, jj) * t0 + G.co(by, ny, 3, jj) * t(e, ii, jj - 1, fx, fy);
+    }
+    if (s != 0.0) {
+      const cplx ex = fld ? ldg(fld + g) : to_cplx(ldg(G.fb + g)), ey = fld ? ldg(fld + G.N + g) : to_cplx(ldg(G.fb + G.N + g));
+      q1 += (s * ey) * G.ld(e + G.N, ii, jj);
+      q2 -= (s * ex) * G.ld(e, ii, jj);
+    }
+  }
+  __device__ __forceinline__ void ww2(int ii, int jj, cplx w[2], cplx h[2], cplx h2[2]) const {
+    w[0] = w[1] = h[0] = h[1] = h2[0] = h2[1] = mk(0.0, 0.0);
+    if (!G.in(ii, jj)) return;
+    const T *v = G.v, *x = G.x;
+    const cplx *c = nullptr;  // no eps term
+    const T *cx = G.cx, *cy = G.cy, *dx = G.dcx, *dy = G.dcy, *ex = c2x, *ey = c2y;
+    cplx a1, a2, b1, b2;
+    cplx q01, q02;  // Q v
+    q(v, ii, jj, cx, cy, cx, cy, nullptr, 1.0, q01, q02);
+    cplx q11 = mk(0.0, 0.0), q12 = mk(0.0, 0.0);  // Q_1 v + Q x
+    q(v, ii, jj, dx, dy, cx, cy, c, 0.0, a1, a2);
+    q(v, ii, jj, cx, cy, dx, dy, G.p1, G.p1 ? 1.0 : 0.0, b1, b2);
+    q11 = a1 + b1;
+    q12 = a2 + b2;
+    q(x, ii, jj, cx, cy, cx, cy, nullptr, 1.0, a1, a2);
+    q11 += a1;
+    q12 += a2;
+    // Q_2 v + Q_1 x + Q x2, Q_2 v = B(c', c') v + Q_c[c''/2] v + Q_p[p''/2] v
+    cplx q21, q22;
+    q(v, ii, jj, dx, dy, dx, dy, p2, p2 ? 0.5 : 0.0, q21, q22);
+    q(v, ii, jj, ex, ey, cx, cy, c, 0.0, a1, a2);
+    q(v, ii, jj, cx, cy, ex, ey, c, 0.0, b1, b2);
+    q21 += 0.5 * (a1 + b1);
+    q22 += 0.5 * (a2 + b2);
+    q(x, ii, jj, dx, dy, cx, cy, c, 0.0, a1, a2);
+    q(x, ii, jj, cx, cy, dx, dy, G.p1, G.p1 ? 1.0 : 0.0, b1, b2);
+    q21 += a1 + b1;
+    q22 += a2 + b2;
+    q(x2, ii, jj, cx, cy, cx, cy, nullptr, 1.0, a1, a2);
+    q21 += a1;
+    q22 += a2;
+    const int nx = G.nx, ny = G.ny;
+    const cplx lfx = G.gx[ii], lbx = G.gx[nx + ii], lfy = G.gy[jj], lby = G.gy[ny + jj];
+    auto d1 = [](cplx l) { return mk(0.0, -l.im); };  // l_1 = -i Im l, l_2 = i Im l
+    auto d2 = [](cplx l) { return mk(0.0, l.im); };
+    const cplx Gf = lfx * lby, Gb = lbx * lfy;
+    const cplx dGf = d1(lfx) * lby + lfx * d1(lby), dGb = d1(lbx) * lfy + lbx * d1(lfy);
+    const cplx eGf = d2(lfx) * lby + d1(lfx) * d1(lby) + lfx * d2(lby), eGb = d2(lbx) * lfy + d1(lbx) * d1(lfy) + lbx * d2(lfy);
+    w[0] = Gf * q02;
+    w[1] = -(Gb * q01);
+    h[0] = dGf * q02 + Gf * q12;
+    h[1] = -(dGb * q01 + Gb * q11);
+    h2[0] = eGf * q02 + dGf * q12 + Gf * q22;
+    h2[1] = -(eGb * q01 + dGb * q11 + Gb * q21);
+  }
+};
+
+// grid (nchunk, B), 256 threads, one mode slot a.q while a.x holds its first-order correction and u.x2 its second-order one:
+// PART 0 writes group 0 of u.partial, PART 1 groups 1-3 (see above)
+template <typename T, typename C, bool HAS_MU, int PART>
+__global__ void __launch_bounds__(256) fourth_scan_kernel(DispArgs<T, C> a, ThirdArgs<T> t, FourthArgs<T> u) {
+  const DerivArgs<T, C> &d = a.d;
+  const int b = blockIdx.y, nx = d.nx, ny = d.ny;
+  const size_t N = (size_t)nx * ny;
+  const bool hp = a.p1 != nullptr;
+  const T *vb = d.vec + (size_t)a.q * d.vstride + (size_t)b * 2 * N, *xb = a.x + (size_t)b * 2 * N, *x2b = u.x2 + (size_t)b * 2 * N;
+  const size_t o4x = (size_t)b * 4 * nx, o4y = (size_t)b * 4 * ny, o3 = (size_t)b * 3 * N;
+  const GroupCell<T, C, HAS_MU> G{vb, xb, d.fields + d.field_bstride * b, d.cx + o4x, d.cy + o4y, d.dcx + o4x, d.dcy + o4y,
+                                  d.gx + (size_t)b * 2 * nx, d.gy + (size_t)b * 2 * ny, hp ? a.p1 + o3 : nullptr, nx, ny, N};
+  const T *cxb = d.cx + o4x, *cyb = d.cy + o4y;
+  auto rows = [&](int k, int ax) -> const T * {  // as in third_scan_kernel, with 6-8 of kFourthTerms
+    const size_t o = ax == 0 ? o4x : o4y;
+    switch (k) {
+      case 1: return (ax == 0 ? d.dcx : d.dcy) + o;
+      case 2: return (ax == 0 ? a.c2x : a.c2y) + o;
+      case 3: return (ax == 0 ? t.c3x : t.c3y) + o;
+      case 4: return (ax == 0 ? t.csx : t.csy) + o;
+      case 5: return (ax == 0 ? t.cdx : t.cdy) + o;
+      case 6: return (ax == 0 ? u.c4x : u.c4y) + o;
+      case 7: return (ax == 0 ? u.qsx : u.qsy) + o;
+      case 8: return (ax == 0 ? u.qdx : u.qdy) + o;
+      default: return nullptr;
+    }
+  };
+  auto fdir = [&](int k) -> const cplx * {
+    if (!hp) return nullptr;
+    switch (k) {
+      case 1: return a.p1 + o3;
+      case 2: return a.p2 + o3;
+      case 3: return t.p3 + o3;
+      case 4: return t.ps + o3;
+      case 5: return t.pd + o3;
+      case 6: return u.p4 + o3;
+      case 7: return u.qs + o3;
+      case 8: return u.qd + o3;
+      default: return nullptr;
+    }
+  };
+  const C *fb = d.fields + d.field_bstride * b;
+  cplx s[9];
+  for (int k = 0; k < 9; ++k) s[k] = mk(0.0, 0.0);
+  for (size_t g = (size_t)blockIdx.x * 256 + threadIdx.x; g < N; g += (size_t)gridDim.x * 256) {
+    const int i = (int)(g / ny), j = (int)(g % ny);
+    if (PART == 0) {
+      cplx yw[2] = {mk(0.0, 0.0), mk(0.0, 0.0)}, yh[2] = {mk(0.0, 0.0), mk(0.0, 0.0)};  // A''''v + 4 A'''x, A'''v
+#pragma unroll 1
+      for (int k = 0; k < (hp ? 26 : 6); ++k) {
+        const ThirdTerm tm = kThirdTerms[k];
+        const CoefRows<T> CX{cxb, rows(tm.cdir, 0), tm.sc, nx}, CY{cyb, rows(tm.cdir, 1), tm.sc, ny};
+        const cplx *dp = fdir(tm.pdir);
+        const PertSite<T, C, HAS_MU> Pv{vb, vb + N, fb, dp, tm.sp, CX, CY, nx, ny, N}, Px{xb, xb + N, fb, dp, tm.sp, CX, CY, nx, ny, N};
+        cplx y1, y2;
+        Pv.apply(i, j, y1, y2);
+        yh[0] += tm.w * y1;
+        yh[1] += tm.w * y2;
+        Px.apply(i, j, y1, y2);
+        yw[0] += (4.0 * tm.w) * y1;
+        yw[1] += (4.0 * tm.w) * y2;
+      }
+#pragma unroll 1
+      for (int k = 0; k < (hp ? 64 : 9); ++k) {
+        const ThirdTerm tm = kFourthTerms[k];
+        const PertSite<T, C, HAS_MU> Pv{vb, vb + N, fb, fdir(tm.pdir), tm.sp, CoefRows<T>{cxb, rows(tm.cdir, 0), tm.sc, nx},
+                                        CoefRows<T>{cyb, rows(tm.cdir, 1), tm.sc, ny}, nx, ny, N};
+        cplx y1, y2;
+        Pv.apply(i, j, y1, y2);
+        yw[0] += tm.w * y1;
+        yw[1] += tm.w * y2;
+      }
+      cplx w[2], h[2];
+      G.ww(i, j, w, h);
+      s[0] += w[0] * yw[0] + w[1] * yw[1];
+      s[1] += h[0] * yh[0] + h[1] * yh[1];
+    } else {
+      const DispTerm *tab2 = hp ? kDispTermsP : kDispTermsC;
+      const cplx lam = u.sc[3 * b + 2];
+      // A''x2 (w), 12 A''x + 24 A'x2 (w_hat), 12 A''v + 24 A'x + 24 (A - lambda) x2 (w_hat2)
+      cplx yw[2] = {mk(0.0, 0.0), mk(0.0, 0.0)}, yh[2] = {mk(0.0, 0.0), mk(0.0, 0.0)}, yh2[2];
+      {
+        const PertSite<T, C, HAS_MU> P0{x2b, x2b + N, fb, nullptr, 0.0, CoefRows<T>{cxb, nullptr, 0.0, nx}, CoefRows<T>{cyb, nullptr, 0.0, ny},
+                                        nx, ny, N};
+        cplx y1, y2;
+        P0.apply(i, j, y1, y2);
+        yh2[0] = 24.0 * (y1 - lam * to_cplx(ldg(x2b + g)));
+        yh2[1] = 24.0 * (y2 - lam * to_cplx(ldg(x2b + N + g)));
+      }
+#pragma unroll 1
+      for (int k = 0; k < (hp ? 13 : 5); ++k) {
+        const DispTerm tm = tab2[k];
+        const CoefRows<T> CX{cxb, rows(tm.cdir, 0), tm.sc, nx}, CY{cyb, rows(tm.cdir, 1), tm.sc, ny};
+        const cplx *dp = fdir(tm.pdir);
+        const PertSite<T, C, HAS_MU> Pv{vb, vb + N, fb, dp, tm.sp, CX, CY, nx, ny, N}, Px{xb, xb + N, fb, dp, tm.sp, CX, CY, nx, ny, N};
+        const PertSite<T, C, HAS_MU> Px2{x2b, x2b + N, fb, dp, tm.sp, CX, CY, nx, ny, N};
+        cplx y1, y2;
+        Pv.apply(i, j, y1, y2);
+        yh2[0] += (12.0 * tm.w2) * y1;
+        yh2[1] += (12.0 * tm.w2) * y2;
+        Px.apply(i, j, y1, y2);
+        yh2[0] += (24.0 * tm.w1) * y1;
+        yh2[1] += (24.0 * tm.w1) * y2;
+        yh[0] += (12.0 * tm.w2) * y1;
+        yh[1] += (12.0 * tm.w2) * y2;
+        Px2.apply(i, j, y1, y2);
+        yh[0] += (24.0 * tm.w1) * y1;
+        yh[1] += (24.0 * tm.w1) * y2;
+        yw[0] += tm.w2 * y1;
+        yw[1] += tm.w2 * y2;
+      }
+      const SecondCell<T, C, HAS_MU> S2{G, x2b, a.c2x + o4x, a.c2y + o4y, hp ? a.p2 + o3 : nullptr};
+      cplx w[2], h[2], h2[2];
+      S2.ww2(i, j, w, h, h2);
+      const cplx e1 = to_cplx(ldg(vb + g)), e2 = to_cplx(ldg(vb + N + g)), x1 = to_cplx(ldg(xb + g)), x2 = to_cplx(ldg(xb + N + g));
+      const cplx z1 = to_cplx(ldg(x2b + g)), z2 = to_cplx(ldg(x2b + N + g));
+      s[2] += h2[0] * yh2[0] + h2[1] * yh2[1];
+      s[3] += w[0] * yw[0] + w[1] * yw[1];
+      s[4] += h[0] * yh[0] + h[1] * yh[1];
+      s[5] += h2[0] * e1 + h2[1] * e2;
+      s[6] += w[0] * z1 + w[1] * z2;
+      s[7] += h2[0] * x1 + h2[1] * x2;
+      s[8] += h[0] * z1 + h[1] * z2;
+    }
+  }
+  // PART 0: slots 0-2 of group 0 hold s[0], s[1], 0; PART 1: groups 1-3 hold s[2..8], 0, 0
+  const int lo = PART == 0 ? 0 : 2, nsum = PART == 0 ? 3 : 9;
+  __shared__ cplx red[9][256];
+#pragma unroll
+  for (int k = 0; k < nsum; ++k) red[k][threadIdx.x] = (lo + k <= (PART == 0 ? 1 : 8)) ? s[lo + k] : mk(0.0, 0.0);
+  __syncthreads();
+  for (int hh = 128; hh > 0; hh >>= 1) {
+    if ((int)threadIdx.x < hh)
+      for (int k = 0; k < nsum; ++k) red[k][threadIdx.x] += red[k][threadIdx.x + hh];
+    __syncthreads();
+  }
+  const int g0 = PART == 0 ? 0 : 1;
+  if ((int)threadIdx.x < nsum)
+    u.partial[(((size_t)b * 4 + g0 + threadIdx.x / 3) * gridDim.x + blockIdx.x) * 3 + threadIdx.x % 3] = red[threadIdx.x][0];
 }
 
 // ------------------------------------------------------------------------------------------------

@@ -250,3 +250,11 @@ def beta3_of(freq, d2n_dfreq2, d3n_dfreq3):
     against the derivatives like in ``dispersion_of``."""
     f = np.asarray(freq, float)
     return (3 * np.real(d2n_dfreq2) + f * np.real(d3n_dfreq3)) / (4 * np.pi**2 * (C0_UM * 1e-6)) * 1e39
+
+
+def beta4_of(freq, d3n_dfreq3, d4n_dfreq4):
+    """Fourth-order dispersion beta4 = d^4 beta / d omega^4 (ps^4/km) of beta = omega n / c, from analytic frequency derivatives
+    of n_eff + i k_eff (``compute_modes_batch(..., derivatives=("freq4",))``): beta4 = (4 Re n''' + f Re n'''') / (8 pi^3 c), c in
+    m/s (1 s^4/m = 1e51 ps^4/km).  ``freq`` broadcasts against the derivatives like in ``dispersion_of``."""
+    f = np.asarray(freq, float)
+    return (4 * np.real(d3n_dfreq3) + f * np.real(d4n_dfreq4)) / (8 * np.pi**3 * (C0_UM * 1e-6)) * 1e51

@@ -109,6 +109,17 @@ class Medium:
         t = self.tensor
         return (t(freq + 2 * h) - 2 * t(freq + h) + 2 * t(freq - h) - t(freq - 2 * h)) / (2 * h**3)
 
+    def d4tensor_dfreq4(self, freq: float) -> np.ndarray:
+        """d^4 eps / df^4 (1/Hz^4) of the 3x3 tensor: zero for a constant medium, a fourth central difference of ``eps(f)`` at
+        f, f +- h, f +- 2h for a dispersive one.  The relative step is 5e-3: the roundoff grows like 16 eps_mach / step^4 (about 3e-6
+        relative to eps at 5e-3, 1e-4 at 2e-3), the truncation error like step^2 / 6 (zero for a quartic eps(f)); the two balance
+        near 5e-3."""
+        if not callable(self.eps):
+            return np.zeros((3, 3), dtype=complex)
+        h = 5e-3 * freq
+        t = self.tensor
+        return (t(freq + 2 * h) - 4 * t(freq + h) + 6 * t(freq) - 4 * t(freq - h) + t(freq - 2 * h)) / h**4
+
 
 def site_medium_from_masks(shape: Tuple[int, int], masks: Sequence[Tuple[np.ndarray, int]]) -> np.ndarray:
     """(3, Nx, Ny) uint16 site map from per-structure inside-masks, drawn in structure order like epsilon_on_grid
@@ -169,6 +180,15 @@ class Section:
         if tuple(sm.shape[1:]) != tuple(shape):
             raise ValueError("Mismatch between 'coords' and 'site_medium' shapes.")
         return sm
+
+    def d4_table(self, freq: float) -> Optional[np.ndarray]:
+        """Every medium's d^4 eps / df^4 at ``freq``, (nmedia, 9) complex128 in the order of ``pack``'s ``eps_table`` (the
+        ``d4eps_table`` of b200ms_problem_ext, the material term of the fourth frequency derivative), or None when no medium is
+        dispersive."""
+        media, _ = self._media()
+        if not any(callable(m.eps) for m in media):
+            return None
+        return np.ascontiguousarray([m.d4tensor_dfreq4(freq).ravel() for m in media], dtype=np.complex128)
 
     def pack(self, freq: float, shape: Optional[Tuple[int, int]] = None, dispersion: bool = False, second: bool = False,
              third: bool = False):

@@ -117,7 +117,12 @@ def compute_modes_batch(
     correction solves (no further solve, by the 2n+1 rule): ``d3n_dfreq3`` (d^3(n_eff + i k_eff)/df^3, 1/Hz^3; NaN where
     ``d2n_dfreq2`` is), ``dispersion_slope`` (dD/d(wavelength), ps/(nm^2 km), ``plugin.dispersion_slope_of``) and ``beta3``
     (d^3 beta / d omega^3, ps^3/km, ``plugin.beta3_of``).  It implies ``"freq2"`` and ``"freq"``, whose outputs do not change;
-    its material term also reads a problem's ``eps_d3freq=`` (d^3 eps_cross / df^3) or a section's callable media.
+    its material term also reads a problem's ``eps_d3freq=`` (d^3 eps_cross / df^3) or a section's callable media.  ``"freq4"``
+    adds the fourth-order dispersion from one more correction solve per mode (the second-order correction of the eigenvector):
+    ``d4n_dfreq4`` (d^4(n_eff + i k_eff)/df^4, 1/Hz^4; NaN for a mode whose first or second correction solve stopped above 100 x
+    the inner tolerance), ``d4n_residual`` (the second solve's final relative residual) and ``beta4`` (d^4 beta / d omega^4,
+    ps^4/km, ``plugin.beta4_of``).  It implies ``"freq3"``, ``"freq2"`` and ``"freq"``, whose outputs do not change; its material
+    term also reads a problem's ``eps_d4freq=`` (d^4 eps_cross / df^4) or a section's callable media.  Tensorial problems raise.
 
     ``left_solve=True`` extends ``"freq"`` and ``"eps"`` to tensorial problems (angled planes, off-diagonal eps such as rotated
     anisotropic crystals), which otherwise raise ``NotImplementedError``: their left eigenvectors come from a second eigen-solve
@@ -133,7 +138,7 @@ def compute_modes_batch(
     if unknown:
         raise ValueError(f"unknown post-processing step(s): {sorted(unknown)}")
     derivatives = tuple(derivatives or ())
-    unknown = set(derivatives) - {"freq", "eps", "freq2", "group_eps", "freq3"}
+    unknown = set(derivatives) - {"freq", "eps", "freq2", "group_eps", "freq3", "freq4"}
     if unknown:
         raise ValueError(f"unknown derivative(s): {sorted(unknown)}")
     if left_solve and not derivatives:
@@ -141,6 +146,9 @@ def compute_modes_batch(
     group_eps = "group_eps" in derivatives
     if group_eps:
         derivatives = derivatives + tuple(d for d in ("eps", "freq2") if d not in derivatives)
+    fourth = "freq4" in derivatives
+    if fourth and "freq3" not in derivatives:
+        derivatives = derivatives + ("freq3",)
     third = "freq3" in derivatives
     if third and "freq2" not in derivatives:
         derivatives = derivatives + ("freq2",)
@@ -172,7 +180,7 @@ def compute_modes_batch(
             incidence=(split is not None or p.get("mu_cross") is not None),  # solver.py:93
             post=post_flags, grid_correction=p.get("grid_correction"), plane_bounds=p.get("plane_bounds"),
             eps_dfreq=p.get("eps_dfreq"), derivatives="freq" in derivatives, eps_d2freq=p.get("eps_d2freq"), second=second,
-            eps_d3freq=p.get("eps_d3freq"), third=third, left_solve=left_solve,
+            eps_d3freq=p.get("eps_d3freq"), third=third, left_solve=left_solve, eps_d4freq=p.get("eps_d4freq"), fourth=fourth,
         )  # fmt: skip
         if split is None and section is None:
             cache[key] = pk.eps
@@ -187,7 +195,7 @@ def compute_modes_batch(
     with h.lock:
         want_eps = "eps" in derivatives
         dkw = dict(want_dfreq="freq" in derivatives, want_deps=want_eps and not left_solve, want_deps_tensor=want_eps and left_solve,
-                   want_d2freq=second, want_group_eps=group_eps, want_d3freq=third) if derivatives else {}
+                   want_d2freq=second, want_group_eps=group_eps, want_d3freq=third, want_d4freq=fourth) if derivatives else {}
         rc, fields, ncs, results = h.solve_batch(packed, want_fields, fields_ptrs, want_flux=("flux" in post or "normalize" in post),
                                                  want_overlaps="overlaps" in post, **dkw)
         flux_out, te_out, ov_out = h.last_flux, h.last_te, h.last_overlaps
@@ -195,6 +203,7 @@ def compute_modes_batch(
         d2_out, d2res_out = (h.last_d2n_dfreq2, h.last_d2n_residual) if second else ([], [])
         gmap_out = h.last_d2n_dfreq_deps if group_eps else []
         d3_out = h.last_d3n_dfreq3 if third else []
+        d4_out, d4res_out = (h.last_d4n_dfreq4, h.last_d4n_residual) if fourth else ([], [])
         err = h.last_error() if rc != _cabi.OK else ""
     if rc != _cabi.OK:
         bad = [i for i in range(len(packed)) if results[i].status != _cabi.OK]
@@ -238,6 +247,12 @@ def compute_modes_batch(
             infos[-1]["d3n_dfreq3"] = d3_out[i]
             infos[-1]["dispersion_slope"] = dispersion_slope_of(fq, dfreq_out[i], d2_out[i], d3_out[i])
             infos[-1]["beta3"] = beta3_of(fq, d2_out[i], d3_out[i])
+        if d4_out:
+            from .plugin import beta4_of  # noqa: PLC0415  (plugin imports this module)
+
+            infos[-1]["d4n_dfreq4"] = d4_out[i]
+            infos[-1]["d4n_residual"] = d4res_out[i]
+            infos[-1]["beta4"] = beta4_of(float(packed[i].struct.freq), d3_out[i], d4_out[i])
     return (out, infos) if return_info else out
 
 
