@@ -267,6 +267,22 @@ typedef struct {
                             solve (needs d4n_dfreq4) */
 } b200ms_result_ext;
 
+/* ---- Permittivity gradient of each mode's group-velocity dispersion (b200ms_solve_batch_ext2; the version stays 211).  No
+   further solve: in t = (f_new - f) / f the corrections x, x2 of the fourth-order pass and the structural w_hat, w_hat2 give
+   v(t) = v + t x + t^2 x2 and w(t) = w + t w_hat + t^2 w_hat2 to second order, and the t^0..t^2 coefficients of
+   w(t)^T A(t) v(t) / w(t)^T v(t) are stationary in all six vectors, so d_g (lambda''/2) is the explicit partial at fixed vectors:
+     d_g lambda_2 = E_2 / D_0 - (E_1 D_1 + E_0 D_2) / D_0^2 + E_0 D_1^2 / D_0^3,   E(t) = chi_a(t) w(t)^T (dA/dp_a(g))(t) v(t)
+   (D_k as for d4n_dfreq4; see DESIGN.md §4).  Same scope as d4n_dfreq4; n_complex, the fields and every other derivative and
+   map do not change when it is asked for.  Indexed like prob / res. ---- */
+typedef struct {
+  double *d2n_dfreq2_deps; /* NULL, or caller-allocated 3*nx*ny*num_modes complex128 (re,im), layout of dn_deps: d(d^2n/df^2) / d eps_aa
+                              (1/Hz^2) of the caller's eps_cross at every Yee site, at fixed d eps / df, d^2 eps / df^2 and PML stretch
+                              (0 at PEC-valued cells).  Needs result.d2n_dfreq_deps and b200ms_result_ext.d4n_dfreq4 (else
+                              B200MS_ERR_ARG); NaN for every cell of a mode where d4n_dfreq4 is NaN.  The gradient of the dispersion D
+                              for a real change of eps: -1e18 f^2 (2 Re d2n_dfreq_deps + f Re d2n_dfreq2_deps) / c0^2 (c0 in um/s).
+                              HOST or DEVICE memory like `fields` */
+} b200ms_result_ext2;
+
 /* Tunables (all have defaults; see DESIGN.md). */
 typedef struct {
   double eig_tol;        /* relative Ritz residual tolerance; default 1.19e-7 = the reference's ARPACK tol (solver.py:20,745);
@@ -371,6 +387,10 @@ int b200ms_solve_batch(b200ms_handle *h, int nprob, const b200ms_problem *prob, 
  * this call with both NULL). */
 int b200ms_solve_batch_ext(b200ms_handle *h, int nprob, const b200ms_problem *prob, b200ms_result *res, const b200ms_problem_ext *pext,
                            const b200ms_result_ext *rext);
+/* b200ms_solve_batch_ext with the dispersion gradient: rext2 is NULL or nprob entries (b200ms_solve_batch_ext is this call with
+ * rext2 NULL). */
+int b200ms_solve_batch_ext2(b200ms_handle *h, int nprob, const b200ms_problem *prob, b200ms_result *res, const b200ms_problem_ext *pext,
+                            const b200ms_result_ext *rext, const b200ms_result_ext2 *rext2);
 
 /* Benchmark / roofline hook: run one of the two hot stencil kernels `nrep` times on `nbatch` device-resident copies
  * of the operator of `prob` and return the mean kernel time (CUDA events on the library stream).

@@ -61,6 +61,10 @@ class ResultExt(C.Structure):
     _fields_ = [("d4n_dfreq4", _dp), ("d4n_residual", _dp)]
 
 
+class ResultExt2(C.Structure):
+    _fields_ = [("d2n_dfreq2_deps", _dp)]
+
+
 class Options(C.Structure):
     _fields_ = [
         ("eig_tol", C.c_double), ("inner_tol", C.c_double), ("ncv", C.c_int), ("max_restarts", C.c_int),
@@ -81,7 +85,7 @@ class Stats(C.Structure):
 
 EXPORTS = [
     "b200ms_version", "b200ms_get_stats", "b200ms_default_options", "b200ms_create", "b200ms_destroy", "b200ms_set_options",
-    "b200ms_last_error", "b200ms_host_alloc", "b200ms_host_free", "b200ms_solve_batch", "b200ms_solve_batch_ext", "b200ms_bench_stencil", "b200ms_debug_schur", "b200ms_debug_setup",
+    "b200ms_last_error", "b200ms_host_alloc", "b200ms_host_free", "b200ms_solve_batch", "b200ms_solve_batch_ext", "b200ms_solve_batch_ext2", "b200ms_bench_stencil", "b200ms_debug_schur", "b200ms_debug_setup",
     "b200ms_debug_hierarchy", "b200ms_debug_batch", "b200ms_debug_apply", "b200ms_debug_vcycle", "b200ms_debug_solve", "b200ms_debug_march2_geometry", "b200ms_debug_post_tables", "b200ms_debug_post_tables_bounded", "b200ms_debug_te_terms", "b200ms_debug_grid_factors", "b200ms_debug_krylov", "b200ms_debug_fields",
 ]  # fmt: skip
 
@@ -121,6 +125,8 @@ def lib():
             L.b200ms_solve_batch.argtypes = [C.c_void_p, C.c_int, C.POINTER(Problem), C.POINTER(Result)]
             L.b200ms_solve_batch_ext.argtypes = [C.c_void_p, C.c_int, C.POINTER(Problem), C.POINTER(Result), C.POINTER(ProblemExt),
                                                  C.POINTER(ResultExt)]
+            L.b200ms_solve_batch_ext2.argtypes = [C.c_void_p, C.c_int, C.POINTER(Problem), C.POINTER(Result), C.POINTER(ProblemExt),
+                                                  C.POINTER(ResultExt), C.POINTER(ResultExt2)]
             L.b200ms_bench_stencil.argtypes = [C.c_void_p, C.POINTER(Problem), C.c_int, C.c_int, C.c_int, C.c_int, _dp, _dp, _dp, _dp]
             L.b200ms_debug_schur.argtypes = [C.c_int, _dp, _dp, _dp]
             L.b200ms_debug_setup.argtypes = [C.POINTER(Problem), _dp, _ip, _dp, _dp, _dp, _dp, _dp]
@@ -373,7 +379,8 @@ class Handle:
             pass
 
     def solve_batch(self, packed, want_fields=True, fields_ptrs=None, want_flux=False, want_overlaps=False, want_dfreq=False, want_deps=False,
-                    want_d2freq=False, want_group_eps=False, want_d3freq=False, want_deps_tensor=False, want_d4freq=False):
+                    want_d2freq=False, want_group_eps=False, want_d3freq=False, want_deps_tensor=False, want_d4freq=False,
+                    want_d2freq2_deps=False):
         """packed: list of PackedProblem.  Returns (rc, fields list | None, n_complex list, Result structs).
 
         ``fields_ptrs``: optional list of raw addresses (host or DEVICE memory, e.g. ``tensor.data_ptr()``) the library
@@ -385,19 +392,23 @@ class Handle:
         correction solve (``last_d3n_dfreq3``); ``want_deps_tensor``: the nine-component d n / d eps of every mode (result.dn_deps_tensor,
         (9, nx, ny, M) arrays in ``last_dn_deps``; not together with ``want_deps``); ``want_d4freq``: d^4 n / df^4 of every mode and the
         residual of its second correction solve (``last_d4n_dfreq4`` / ``last_d4n_residual``, b200ms_solve_batch_ext; needs
-        ``want_d3freq``)."""
+        ``want_d3freq``); ``want_d2freq2_deps``: d(d^2n/df^2) / d eps of every mode from the corrections of both passes
+        (``last_d2n_dfreq2_deps``, b200ms_solve_batch_ext2; needs ``want_group_eps`` and ``want_d4freq``)."""
         if want_deps and want_deps_tensor:
             raise ValueError("want_deps and want_deps_tensor fill the same list: ask for one of them")
         if want_d4freq and not want_d3freq:
             raise ValueError("want_d4freq needs want_d3freq: the fourth derivative is formed from the third-order pass")
+        if want_d2freq2_deps and not (want_group_eps and want_d4freq):
+            raise ValueError("want_d2freq2_deps needs want_group_eps and want_d4freq: the map is formed from both passes' corrections")
         n = len(packed)
         probs = (Problem * n)(*[p.struct for p in packed])
         results = (Result * n)()
         fields, ncs = [], []
         self.last_flux, self.last_te, self.last_overlaps, self.last_dn_dfreq, self.last_dn_deps = [], [], [], [], []
         self.last_d2n_dfreq2, self.last_d2n_residual, self.last_d2n_dfreq_deps, self.last_d3n_dfreq3 = [], [], [], []
-        self.last_d4n_dfreq4, self.last_d4n_residual = [], []
+        self.last_d4n_dfreq4, self.last_d4n_residual, self.last_d2n_dfreq2_deps = [], [], []
         rext = (ResultExt * n)() if want_d4freq else None
+        rext2 = (ResultExt2 * n)() if want_d2freq2_deps else None
         for i, p in enumerate(packed):
             nc = np.zeros(p.num_modes, dtype=np.complex128)
             ncs.append(nc)
@@ -434,6 +445,10 @@ class Handle:
                 self.last_d4n_residual.append(r)
                 rext[i].d4n_dfreq4 = _ptr(d.view(np.float64))
                 rext[i].d4n_residual = _ptr(r)
+            if want_d2freq2_deps:
+                d = np.zeros((3, p.nx, p.ny, p.num_modes), dtype=np.complex128)
+                self.last_d2n_dfreq2_deps.append(d)
+                rext2[i].d2n_dfreq2_deps = _ptr(d.view(np.float64))
             if want_flux:
                 fl, te = np.zeros(p.num_modes), np.zeros(p.num_modes)
                 self.last_flux.append(fl)
@@ -455,7 +470,10 @@ class Handle:
                 results[i].fields = None
         if want_d4freq:
             pext = (ProblemExt * n)(*[p.ext for p in packed])
-            rc = lib().b200ms_solve_batch_ext(self._h, n, probs, results, pext, rext)
+            if want_d2freq2_deps:
+                rc = lib().b200ms_solve_batch_ext2(self._h, n, probs, results, pext, rext, rext2)
+            else:
+                rc = lib().b200ms_solve_batch_ext(self._h, n, probs, results, pext, rext)
         else:
             rc = lib().b200ms_solve_batch(self._h, n, probs, results)
         return rc, (fields if (want_fields and fields_ptrs is None) else None), ncs, results

@@ -76,6 +76,7 @@ struct b200ms_handle {
   b200ms_stats stats;
   const b200ms_problem_ext *pext = nullptr;  // the fourth-order arrays of the b200ms_solve_batch_ext call in progress, or null
   const b200ms_result_ext *rext = nullptr;
+  const b200ms_result_ext2 *rext2 = nullptr;  // the dispersion-gradient maps of a b200ms_solve_batch_ext2 call in progress, or null
 };
 
 extern "C" int b200ms_version(void) { return B200MS_VERSION; }
@@ -1053,8 +1054,10 @@ void tensor_derivative_pass(b200ms_handle *h, BatchSolver<T, C, P, PC> &S, const
 // sums w_hat^T v and writes slot q of the map from the same x; with result.d3n_dfreq3, third_scan_kernel sums the six
 // products of lambda''' from the same x.  With b200ms_result_ext.d4n_dfreq4 (which needs d3n_dfreq3), fourth_rhs_kernel then
 // writes r2 from the same x, a second correction solve (A - lambda_q) x2 = r2 runs at the same shift, and fourth_scan_kernel
-// sums the products of lambda''''.  It writes its own buffers, the first four slots of the outer Krylov basis and the inner
-// solver's scratch -- nothing the fields, the post-processing or the warm start read.
+// sums the products of lambda''''.  With b200ms_result_ext2.d2n_dfreq2_deps (which needs d2n_dfreq_deps and d4n_dfreq4),
+// disp_grad_kernel then writes slot q of the map d_g (d^2n/df^2) from the same x and x2.  It writes its own buffers, the
+// first four slots of the outer Krylov basis and the inner solver's scratch -- nothing the fields, the post-processing or the
+// warm start read.
 template <typename T, typename C, typename P, typename PC>
 void dispersion_pass(b200ms_handle *h, BatchSolver<T, C, P, PC> &S, const std::vector<const ProblemSetup *> &ps, const std::vector<int> &ids,
                      const Window &W, const b200ms_problem *prob, b200ms_result *res, const std::vector<cd> &nsorted,
@@ -1062,7 +1065,7 @@ void dispersion_pass(b200ms_handle *h, BatchSolver<T, C, P, PC> &S, const std::v
   const int B = (int)ids.size(), k = S.k, nx = S.nx, ny = S.ny;
   const size_t N = (size_t)nx * ny;
   std::vector<char> skip(B), skip4(B, 1);
-  bool any_mat = false, any_gmap = false, any_third = false, any_fourth = false;
+  bool any_mat = false, any_gmap = false, any_third = false, any_fourth = false, any_dgrad = false;
   for (int b = 0; b < B; ++b) {
     const b200ms_problem &p = prob[W.i0 + ids[b]];
     const b200ms_result &rb = res[W.i0 + ids[b]];
@@ -1071,6 +1074,7 @@ void dispersion_pass(b200ms_handle *h, BatchSolver<T, C, P, PC> &S, const std::v
     any_third = any_third || rb.d3n_dfreq3;
     skip4[b] = (h->rext && h->rext[W.i0 + ids[b]].d4n_dfreq4) ? 0 : 1;
     any_fourth = any_fourth || !skip4[b];
+    any_dgrad = any_dgrad || (h->rext2 && h->rext2[W.i0 + ids[b]].d2n_dfreq2_deps);
     any_mat = any_mat || (p.eps ? (p.eps_dfreq || p.eps_d2freq) : (p.section->deps_table || p.section->d2eps_table));
   }
   for (int b = 0; b < B && any_third; ++b) {  // the third-order terms also read eps'''
@@ -1177,6 +1181,14 @@ void dispersion_pass(b200ms_handle *h, BatchSolver<T, C, P, PC> &S, const std::v
     end += align256((size_t)B * 4 * nch * 3 * sizeof(cplx));
     o_fsum = end;
     end += align256((size_t)B * 12 * sizeof(cplx));
+  }
+  // dispersion-gradient pass: (beta_0, beta_1, beta_2) per problem and the map [B][3][N][M]
+  size_t o_dbeta = 0, o_dmap = 0;
+  if (any_dgrad) {
+    o_dbeta = end;
+    end += align256((size_t)B * 3 * sizeof(cplx));
+    o_dmap = end;
+    end += align256((size_t)B * 3 * N * k * sizeof(cplx));
   }
   h->disp.reserve(end + 256);
   unsigned char *base = h->disp.p;
@@ -1425,15 +1437,42 @@ void dispersion_pass(b200ms_handle *h, BatchSolver<T, C, P, PC> &S, const std::v
         re.d4n_dfreq4[2 * q + 1] = d4n.imag();
         if (re.d4n_residual) re.d4n_residual[q] = resv2[b];
       }
+      if (any_dgrad) {  // d_g (d^2n/df^2) of slot q while x and x2 still hold its corrections
+        std::vector<cplx> bg((size_t)B * 3);
+        for (int b = 0; b < B; ++b) {
+          const cplx *s = sv.data() + (size_t)b * 3, *t = sx.data() + (size_t)b * 3, *u = s3.data() + (size_t)b * 6, *z = s4.data() + (size_t)b * 12;
+          const cd D0 = zc(s[0]), D1 = zc(u[0]) + zc(t[0]), D2 = zc(z[6]) + zc(u[1]) + zc(z[7]), l1 = zc(sc[3 * b]), l2 = zc(sc[3 * b + 1]);
+          const double f = freq[b];
+          const cd sn = nsorted[(size_t)b * k + q], s1 = -l1 / (2.0 * sn), s2 = -(l2 + 2.0 * s1 * s1) / (2.0 * sn);
+          // coefficients of (E_0, E_1, E_2) in d_g lambda, d_g lambda', d_g lambda'' (scaled), then the chain to s'' = n'' / knorm
+          cd dl[3] = {1.0 / D0, 0.0, 0.0}, dl1[3] = {-D1 / (D0 * D0), 1.0 / D0, 0.0};
+          cd dl2[3] = {2.0 * (D1 * D1 / (D0 * D0 * D0) - D2 / (D0 * D0)), -2.0 * D1 / (D0 * D0), 2.0 / D0};
+          for (int e = 0; e < 3; ++e) {
+            const cd ds = -dl[e] / (2.0 * sn), ds1 = -(dl1[e] + 2.0 * s1 * ds) / (2.0 * sn);
+            cd be = ps[b]->knorm * (-(dl2[e] + 4.0 * s1 * ds1 + 2.0 * s2 * ds) / (2.0 * sn)) / (f * f);
+            if (skip4[b] || std::abs(D0) == 0 || !(resv[b] <= 100.0 * tol) || !(resv2[b] <= 100.0 * tol)) be = cd(std::nan(""), std::nan(""));
+            bg[3 * b + e] = mk(be.real(), be.imag());
+          }
+        }
+        cplx *dbeta_g = reinterpret_cast<cplx *>(base + o_dbeta), *dmap = reinterpret_cast<cplx *>(base + o_dmap);
+        CUDA_CHECK(cudaMemcpyAsync(dbeta_g, bg.data(), bg.size() * sizeof(cplx), cudaMemcpyHostToDevice, st));
+        const dim3 blk(64, 4), grd((ny + 63) / 64, (nx + 3) / 4, B);
+        if (S.has_mu) disp_grad_kernel<T, C, true><<<grd, blk, 0, st>>>(a, fa, dbeta_g, dmap);
+        else disp_grad_kernel<T, C, false><<<grd, blk, 0, st>>>(a, fa, dbeta_g, dmap);
+        CUDA_CHECK(cudaGetLastError());
+        h->stats.launches += 1;
+      }
     }
   }
   S.reset_sigma();
   if (!any_gmap) return;
-  const cplx *gmap = reinterpret_cast<const cplx *>(base + o_gmap);
+  const cplx *gmap = reinterpret_cast<const cplx *>(base + o_gmap), *dmap = reinterpret_cast<const cplx *>(base + o_dmap);
   for (int b = 0; b < B; ++b) {
     b200ms_result &r = res[W.i0 + ids[b]];
     if (r.d2n_dfreq_deps)
       CUDA_CHECK(cudaMemcpyAsync(r.d2n_dfreq_deps, gmap + (size_t)b * 3 * N * k, 3 * N * k * sizeof(cplx), cudaMemcpyDefault, st));
+    double *m2 = h->rext2 ? h->rext2[W.i0 + ids[b]].d2n_dfreq2_deps : nullptr;
+    if (m2) CUDA_CHECK(cudaMemcpyAsync(m2, dmap + (size_t)b * 3 * N * k, 3 * N * k * sizeof(cplx), cudaMemcpyDefault, st));
   }
   CUDA_CHECK(cudaStreamSynchronize(st));
 }
@@ -1799,9 +1838,16 @@ static int solve_batch_impl(b200ms_handle *h, int nprob, const b200ms_problem *p
   return first_err;
 }
 
-extern "C" int b200ms_solve_batch_ext(b200ms_handle *h, int nprob, const b200ms_problem *prob, b200ms_result *res,
-                                      const b200ms_problem_ext *pext, const b200ms_result_ext *rext) {
+extern "C" int b200ms_solve_batch_ext2(b200ms_handle *h, int nprob, const b200ms_problem *prob, b200ms_result *res,
+                                       const b200ms_problem_ext *pext, const b200ms_result_ext *rext, const b200ms_result_ext2 *rext2) {
   if (!h || nprob < 0 || (nprob > 0 && (!prob || !res))) return B200MS_ERR_ARG;
+  for (int i = 0; i < nprob && rext2; ++i) {
+    if (rext2[i].d2n_dfreq2_deps && !(res[i].d2n_dfreq_deps && rext && rext[i].d4n_dfreq4)) {  // formed from both passes' corrections
+      h->err = "d2n_dfreq2_deps needs d2n_dfreq_deps and d4n_dfreq4 of the same problem";
+      res[i].status = B200MS_ERR_ARG;
+      return B200MS_ERR_ARG;
+    }
+  }
   for (int i = 0; i < nprob && rext; ++i) {
     if (rext[i].d4n_dfreq4 && !res[i].d3n_dfreq3) {  // lambda'''' is formed from the third-order pass of the same slot
       h->err = "d4n_dfreq4 needs d3n_dfreq3 of the same problem";
@@ -1816,14 +1862,21 @@ extern "C" int b200ms_solve_batch_ext(b200ms_handle *h, int nprob, const b200ms_
   }
   h->pext = pext;
   h->rext = rext;
+  h->rext2 = rext2;
   const int rc = solve_batch_impl(h, nprob, prob, res);
   h->pext = nullptr;
   h->rext = nullptr;
+  h->rext2 = nullptr;
   return rc;
 }
 
+extern "C" int b200ms_solve_batch_ext(b200ms_handle *h, int nprob, const b200ms_problem *prob, b200ms_result *res,
+                                      const b200ms_problem_ext *pext, const b200ms_result_ext *rext) {
+  return b200ms_solve_batch_ext2(h, nprob, prob, res, pext, rext, nullptr);
+}
+
 extern "C" int b200ms_solve_batch(b200ms_handle *h, int nprob, const b200ms_problem *prob, b200ms_result *res) {
-  return b200ms_solve_batch_ext(h, nprob, prob, res, nullptr, nullptr);
+  return b200ms_solve_batch_ext2(h, nprob, prob, res, nullptr, nullptr, nullptr);
 }
 
 // ---- benchmark hook -----------------------------------------------------------------------------------

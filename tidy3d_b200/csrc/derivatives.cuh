@@ -996,6 +996,120 @@ __global__ void __launch_bounds__(256) fourth_scan_kernel(DispArgs<T, C> a, Thir
 }
 
 // ------------------------------------------------------------------------------------------------
+// Dispersion-gradient pass: d_g (d^2n/df^2), the permittivity gradient of each mode's second frequency derivative, from the
+// corrections x, x2 of the fourth-order pass (oracle/mode_dispersion_gradient.py is the float64 model).  In t = (f_new - f) / f,
+// with v(t) = v + t x + t^2 x2 and w(t) = w + t w_hat + t^2 w_hat2, the t^0..t^2 coefficients of N/D are stationary in all six
+// vectors, so d_g lambda_2 (lambda_2 = lambda''/2) is [t^2] of E(t) / D(t) at fixed vectors, E(t) = chi_a(t) D_a(t)(w(t), v(t)):
+//   E_0 = chi D(w, v),   E_1 = chi [D(w_hat, v) + D(w, x) + D_1(w, v)] + chi_1 D(w, v),
+//   E_2 = chi [D(w_hat2, v) + D(w_hat, x) + D(w, x2) + D_1(w_hat, v) + D_1(w, x) + D_2(w, v)] + chi_1 [D(w_hat, v) + D(w, x) + D_1(w, v)]
+//         + chi_2 D(w, v),
+// D_k the t^k coefficient of the form at (c + t c' + t^2 c''/2, p + t p' + t^2 p''/2): D_1 = [D(c+c') - D(c-c')]/2 + [D(p+p') - D(p-p')]/2,
+// D_2 = [D(c+c') + D(c-c')]/2 - D + [D(c+c''/2) - D(c-c''/2)]/2 + [D(p+p''/2) - D(p-p''/2)]/2 + [D(c'+, p'+) - D(c'+, p'-) - D(c'-, p'+)
+// + D(c'-, p'-)]/4, all exact with unit steps.  chi_zz(t) = -je iez(t)^2: chi_1 = -2 je iez iez', chi_2 = -je (2 iez iez''/2 + iez'^2).
+// The host folds d_g lambda_2 = E_2/D_0 - (E_1 D_1 + E_0 D_2)/D_0^2 + E_0 D_1^2/D_0^3 and the chain to n'' into three scalars per
+// problem, so map[b][a][g][q] = beta_0 E_0 + beta_1 E_1 + beta_2 E_2 (NaN where d4n_dfreq4 is NaN).
+// ------------------------------------------------------------------------------------------------
+
+// grid like deriv_map_kernel for one mode slot a.q while a.x holds its first-order correction and u.x2 its second-order one;
+// beta: [B][3]; map: [B][3][N][M]
+template <typename T, typename C, bool HAS_MU>
+__global__ void __launch_bounds__(256) disp_grad_kernel(DispArgs<T, C> a, FourthArgs<T> u, const cplx *beta, cplx *map) {
+  const DerivArgs<T, C> &d = a.d;
+  const int nx = d.nx, ny = d.ny, M = d.num_modes, b = blockIdx.z;
+  const size_t N = (size_t)nx * ny;
+  const int j = blockIdx.x * 64 + threadIdx.x, i = blockIdx.y * 4 + threadIdx.y;
+  if (i >= nx || j >= ny) return;
+  const bool hp = a.p1 != nullptr;
+  const T *vb = d.vec + (size_t)a.q * d.vstride + (size_t)b * 2 * N, *xb = a.x + (size_t)b * 2 * N, *x2b = u.x2 + (size_t)b * 2 * N;
+  const size_t o4x = (size_t)b * 4 * nx, o4y = (size_t)b * 4 * ny, o3 = (size_t)b * 3 * N;
+  const GroupCell<T, C, HAS_MU> G{vb, xb, d.fields + d.field_bstride * b, d.cx + o4x, d.cy + o4y, d.dcx + o4x, d.dcy + o4y,
+                                  d.gx + (size_t)b * 2 * nx, d.gy + (size_t)b * 2 * ny, hp ? a.p1 + o3 : nullptr, nx, ny, N};
+  GroupCell<T, C, HAS_MU> G2 = G;  // the same site with the directions c'' and p'' in place of c' and p'
+  G2.dcx = a.c2x + o4x;
+  G2.dcy = a.c2y + o4y;
+  G2.p1 = hp ? a.p2 + o3 : nullptr;
+  const SecondCell<T, C, HAS_MU> S2{G, x2b, a.c2x + o4x, a.c2y + o4y, hp ? a.p2 + o3 : nullptr};
+  const int di[7] = {0, -1, 0, 1, 1, 0, -1}, dj[7] = {0, 0, -1, 0, -1, 1, 1};
+  // w_hat and w_hat2 stream over the stencil: z of w_hat at c, c + c', c - c' and of w_hat2 at c, and both at (i, j)
+  cplx hz[3][3], h2z[3], h0[2], h20[2], un[2];
+  for (int k = 0; k < 3; ++k) hz[0][k] = hz[1][k] = hz[2][k] = h2z[k] = mk(0.0, 0.0);
+#pragma unroll
+  for (int s = 0; s < 7; ++s) {
+    cplx hs[2], h2s[2];
+    S2.ww2(i + di[s], j + dj[s], un, hs, h2s);
+    G.zadd(s, i, j, hs[0], hs[1], 0.0, hz[0]);
+    G.zadd(s, i, j, hs[0], hs[1], 1.0, hz[1]);
+    G.zadd(s, i, j, hs[0], hs[1], -1.0, hz[2]);
+    G.zadd(s, i, j, h2s[0], h2s[1], 0.0, h2z);
+    if (s == 0) h0[0] = hs[0], h0[1] = hs[1], h20[0] = h2s[0], h20[1] = h2s[1];
+  }
+  cplx b1[3], b2[3], t[3], t2[3];  // the brackets of E_1 and E_2
+  G.forms_z(i, j, hz[0], h0[0], h0[1], vb, 0.0, 0.0, b1);
+  G.forms_z(i, j, h2z, h20[0], h20[1], vb, 0.0, 0.0, b2);
+  G.forms_z(i, j, hz[0], h0[0], h0[1], xb, 0.0, 0.0, t);
+  for (int k = 0; k < 3; ++k) b2[k] += t[k];
+  G.forms_z(i, j, hz[1], h0[0], h0[1], vb, 1.0, 0.0, t);  // D_1(w_hat, v)
+  G.forms_z(i, j, hz[2], h0[0], h0[1], vb, -1.0, 0.0, t2);
+  for (int k = 0; k < 3; ++k) b2[k] += 0.5 * (t[k] - t2[k]);
+  if (hp) {
+    G.forms_z(i, j, hz[0], h0[0], h0[1], vb, 0.0, 1.0, t);
+    G.forms_z(i, j, hz[0], h0[0], h0[1], vb, 0.0, -1.0, t2);
+    for (int k = 0; k < 3; ++k) b2[k] += 0.5 * (t[k] - t2[k]);
+  }
+  // then the w stencil is kept for the forms of w
+  cplx W[7][2], d0[3];
+#pragma unroll
+  for (int s = 0; s < 7; ++s) G.ww(i + di[s], j + dj[s], W[s], un);
+  G.forms(i, j, W, vb, 0.0, 0.0, d0);
+  G.forms(i, j, W, xb, 0.0, 0.0, t);
+  for (int k = 0; k < 3; ++k) b1[k] += t[k];
+  G.forms(i, j, W, x2b, 0.0, 0.0, t);
+  for (int k = 0; k < 3; ++k) b2[k] += t[k] - d0[k];  // - D(w, v) of D_cc[c', c']
+#pragma unroll 1
+  for (int s = 0; s < (hp ? 4 : 2); ++s) {  // D_1(w, v), D_1(w, x) and D_cc[c', c'](w, v): +-c', then +-p'
+    const double st = (s & 1) ? -1.0 : 1.0, sc = s < 2 ? st : 0.0, sp = s < 2 ? 0.0 : st;
+    G.forms(i, j, W, vb, sc, sp, t);
+    G.forms(i, j, W, xb, sc, sp, t2);
+    for (int k = 0; k < 3; ++k) {
+      b1[k] += (0.5 * st) * t[k];
+      b2[k] += (0.5 * st) * t2[k];
+      if (s < 2) b2[k] += 0.5 * t[k];
+    }
+  }
+#pragma unroll 1
+  for (int s = 0; s < (hp ? 4 : 2); ++s) {  // D_c[c''/2](w, v), then D_p[p''/2](w, v)
+    const double st = (s & 1) ? -0.5 : 0.5;
+    G2.forms(i, j, W, vb, s < 2 ? st : 0.0, s < 2 ? 0.0 : st, t);
+    for (int k = 0; k < 3; ++k) b2[k] += st * t[k];
+  }
+#pragma unroll 1
+  for (int s = 0; s < (hp ? 4 : 0); ++s) {  // D_cp[c', p'](w, v)
+    const double sc = (s & 2) ? -1.0 : 1.0, sp = (s & 1) ? -1.0 : 1.0;
+    G.forms(i, j, W, vb, sc, sp, t);
+    for (int k = 0; k < 3; ++k) b2[k] += (0.25 * sc * sp) * t[k];
+  }
+  const size_t g = (size_t)i * ny + j;
+  const cplx iz = to_cplx(ldg(G.fb + 2 * N + g));
+  const double je = d.jz_e ? d.jz_e[(size_t)b * d.jz_len + (d.jz_axis == 0 ? i : j)] : 1.0;
+  const cplx chi[3] = {mk(1.0 / je, 0.0), mk(1.0 / je, 0.0), -(iz * iz) * je};
+  const cplx iz1 = hp ? ldg(a.p1 + o3 + 2 * N + g) : mk(0.0, 0.0), iz2 = hp ? 0.5 * ldg(a.p2 + o3 + 2 * N + g) : mk(0.0, 0.0);
+  const cplx chi1 = -2.0 * je * (iz * iz1), chi2 = -je * (2.0 * (iz * iz2) + iz1 * iz1);
+  const cplx be0 = beta[3 * b], be1 = beta[3 * b + 1], be2 = beta[3 * b + 2];
+  const double pec = 0.9 * 1e8;  // PEC-valued input, as eps_grad
+  const bool is_pec[3] = {abs2(to_cplx(ldg(G.fb + g))) >= pec * pec, abs2(to_cplx(ldg(G.fb + N + g))) >= pec * pec, abs2(iz) * pec * pec <= 1.0};
+  cplx *o = map + (size_t)b * 3 * N * M;
+  for (int k = 0; k < 3; ++k) {
+    cplx e0 = chi[k] * d0[k], e1 = chi[k] * b1[k], e2 = chi[k] * b2[k];
+    if (k == 2) {
+      e1 += chi1 * d0[k];
+      e2 += chi1 * b1[k] + chi2 * d0[k];
+    }
+    if (is_pec[k]) e0 = e1 = e2 = mk(0.0, 0.0);
+    o[((size_t)k * N + g) * M + a.q] = be0 * e0 + be1 * e1 + be2 * e2;
+  }
+}
+
+// ------------------------------------------------------------------------------------------------
 // Tensorial problems: first-order derivatives of the eigenvalue n of mat = msign (-i) M (oracle/tensor_derivatives.py is the
 // float64 model) from the sorted right Ritz vectors u and the left ones w of the transposed Krylov-Schur pass, paired mode by
 // mode (api.cu).  dn = msign (-i) w^T (dM) u / w^T u.  M has degree <= 2 in the 1-D coefficients, so f dM/df u is exactly

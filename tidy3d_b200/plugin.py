@@ -234,6 +234,14 @@ def dispersion_of(freq, dn_dfreq, d2n_dfreq2):
     return -1e18 * f**2 * (2 * np.real(dn_dfreq) + f * np.real(d2n_dfreq2)) / C0_UM**2
 
 
+def dispersion_gradient_of(freq, d2n_dfreq_deps, d2n_dfreq2_deps):
+    """Permittivity gradient of the group-velocity dispersion (ps/(nm km) per unit eps) from the maps of
+    ``compute_modes_batch(..., derivatives=("disp_eps",))``: -1e18 f^2 (2 Re d(n')/d eps + f Re d(n'')/d eps) / c0^2, the gradient of
+    ``dispersion_of`` for a real change of eps at fixed d eps / df and d^2 eps / df^2.  ``freq`` broadcasts against the maps."""
+    f = np.asarray(freq, float)
+    return -1e18 * f**2 * (2 * np.real(d2n_dfreq_deps) + f * np.real(d2n_dfreq2_deps)) / C0_UM**2
+
+
 def dispersion_slope_of(freq, dn_dfreq, d2n_dfreq2, d3n_dfreq3):
     """Dispersion slope S = dD / d(wavelength) (ps/(nm^2 km)) from analytic frequency derivatives of n_eff + i k_eff
     (``compute_modes_batch(..., derivatives=("freq3",))``): dD/df = -1e18 (4 f Re n' + 5 f^2 Re n'' + f^3 Re n''') / c0^2 (c0 in

@@ -122,7 +122,12 @@ def compute_modes_batch(
     ``d4n_dfreq4`` (d^4(n_eff + i k_eff)/df^4, 1/Hz^4; NaN for a mode whose first or second correction solve stopped above 100 x
     the inner tolerance), ``d4n_residual`` (the second solve's final relative residual) and ``beta4`` (d^4 beta / d omega^4,
     ps^4/km, ``plugin.beta4_of``).  It implies ``"freq3"``, ``"freq2"`` and ``"freq"``, whose outputs do not change; its material
-    term also reads a problem's ``eps_d4freq=`` (d^4 eps_cross / df^4) or a section's callable media.  Tensorial problems raise.
+    term also reads a problem's ``eps_d4freq=`` (d^4 eps_cross / df^4) or a section's callable media.  ``"disp_eps"`` adds the
+    permittivity gradient of the group-velocity dispersion from the corrections of ``"group_eps"`` and ``"freq4"`` (no further
+    solve): ``d2n_dfreq2_deps`` (3, Nx, Ny, M), d(d^2n/df^2) / d eps_{xx,yy,zz} (1/Hz^2) at every Yee site at fixed d eps / df,
+    d^2 eps / df^2 and PML stretch (NaN where ``d4n_dfreq4`` is), and ``dispersion_deps`` (ps/(nm km) per unit eps,
+    ``plugin.dispersion_gradient_of``), the gradient of ``dispersion`` for a real change of eps.  It implies ``"group_eps"`` and
+    ``"freq4"``, whose outputs do not change.  Tensorial problems raise.
 
     ``left_solve=True`` extends ``"freq"`` and ``"eps"`` to tensorial problems (angled planes, off-diagonal eps such as rotated
     anisotropic crystals), which otherwise raise ``NotImplementedError``: their left eigenvectors come from a second eigen-solve
@@ -138,11 +143,14 @@ def compute_modes_batch(
     if unknown:
         raise ValueError(f"unknown post-processing step(s): {sorted(unknown)}")
     derivatives = tuple(derivatives or ())
-    unknown = set(derivatives) - {"freq", "eps", "freq2", "group_eps", "freq3", "freq4"}
+    unknown = set(derivatives) - {"freq", "eps", "freq2", "group_eps", "freq3", "freq4", "disp_eps"}
     if unknown:
         raise ValueError(f"unknown derivative(s): {sorted(unknown)}")
     if left_solve and not derivatives:
         raise ValueError("left_solve=True serves derivatives=(\"freq\", \"eps\") of tensorial problems: ask for derivatives as well")
+    disp_eps = "disp_eps" in derivatives
+    if disp_eps:
+        derivatives = derivatives + tuple(d for d in ("group_eps", "freq4") if d not in derivatives)
     group_eps = "group_eps" in derivatives
     if group_eps:
         derivatives = derivatives + tuple(d for d in ("eps", "freq2") if d not in derivatives)
@@ -195,7 +203,8 @@ def compute_modes_batch(
     with h.lock:
         want_eps = "eps" in derivatives
         dkw = dict(want_dfreq="freq" in derivatives, want_deps=want_eps and not left_solve, want_deps_tensor=want_eps and left_solve,
-                   want_d2freq=second, want_group_eps=group_eps, want_d3freq=third, want_d4freq=fourth) if derivatives else {}
+                   want_d2freq=second, want_group_eps=group_eps, want_d3freq=third, want_d4freq=fourth,
+                   want_d2freq2_deps=disp_eps) if derivatives else {}
         rc, fields, ncs, results = h.solve_batch(packed, want_fields, fields_ptrs, want_flux=("flux" in post or "normalize" in post),
                                                  want_overlaps="overlaps" in post, **dkw)
         flux_out, te_out, ov_out = h.last_flux, h.last_te, h.last_overlaps
@@ -204,6 +213,7 @@ def compute_modes_batch(
         gmap_out = h.last_d2n_dfreq_deps if group_eps else []
         d3_out = h.last_d3n_dfreq3 if third else []
         d4_out, d4res_out = (h.last_d4n_dfreq4, h.last_d4n_residual) if fourth else ([], [])
+        dmap_out = h.last_d2n_dfreq2_deps if disp_eps else []
         err = h.last_error() if rc != _cabi.OK else ""
     if rc != _cabi.OK:
         bad = [i for i in range(len(packed)) if results[i].status != _cabi.OK]
@@ -253,6 +263,11 @@ def compute_modes_batch(
             infos[-1]["d4n_dfreq4"] = d4_out[i]
             infos[-1]["d4n_residual"] = d4res_out[i]
             infos[-1]["beta4"] = beta4_of(float(packed[i].struct.freq), d3_out[i], d4_out[i])
+        if dmap_out:
+            from .plugin import dispersion_gradient_of  # noqa: PLC0415  (plugin imports this module)
+
+            infos[-1]["d2n_dfreq2_deps"] = dmap_out[i]
+            infos[-1]["dispersion_deps"] = dispersion_gradient_of(float(packed[i].struct.freq), gmap_out[i], dmap_out[i])
     return (out, infos) if return_info else out
 
 

@@ -6,11 +6,14 @@
   group_eps    -- derivatives=("group_eps",): the same plus the group-index gradient map from the same correction solves;
   analytic_tod -- derivatives=("freq3",): the dispersion pass plus the third-order dispersion from the same correction solves;
   analytic_fod -- derivatives=("freq4",): the same plus the fourth-order dispersion from one more correction solve per mode;
+  fod_group_eps -- derivatives=("freq4", "group_eps"): the fourth-order pass together with the group-index gradient map;
+  disp_eps     -- derivatives=("disp_eps",): the same plus the dispersion gradient map from the corrections of both passes;
   fd3          -- three solves per frequency at f(1 -/+ step) and f, n_group and dispersion by plugin.group_index (the reference's path).
 Prints one JSON line: solves/s, frequencies-with-group-index/s, frequencies-with-dispersion/s, the device time the derivative
 and dispersion passes add per problem, the time the group-index gradient map adds per problem (group_eps - gvd_eps), the time the third-order terms add per
 problem (analytic_tod - analytic_gvd), the time the fourth-order terms add per problem (analytic_fod - analytic_tod) and the
-inner iterations of their second-order correction solves per mode, the correction solves' inner iterations per mode, the largest differences against fd3 and
+inner iterations of their second-order correction solves per mode, the time the dispersion gradient map adds per problem
+(disp_eps - fod_group_eps), the correction solves' inner iterations per mode, the largest differences against fd3 and
 the derivative pass's algorithmic bytes against the 3.35 TB/s HBM3 data-sheet figure, with the card name and power limit read
 in the same run.
 
@@ -69,6 +72,8 @@ def main():
         "group_eps": lambda: compute_modes_batch(probs(wl.freqs), handle=h, want_fields=False, return_info=True, derivatives=("group_eps",)),
         "analytic_tod": lambda: compute_modes_batch(probs(wl.freqs), handle=h, want_fields=False, return_info=True, derivatives=("freq3",)),
         "analytic_fod": lambda: compute_modes_batch(probs(wl.freqs), handle=h, want_fields=False, return_info=True, derivatives=("freq4",)),
+        "fod_group_eps": lambda: compute_modes_batch(probs(wl.freqs), handle=h, want_fields=False, return_info=True, derivatives=("freq4", "group_eps")),
+        "disp_eps": lambda: compute_modes_batch(probs(wl.freqs), handle=h, want_fields=False, return_info=True, derivatives=("disp_eps",)),
         "fd3": lambda: compute_modes_batch(probs(f3), handle=h, want_fields=False, return_info=True),
     }
     for fn in arms.values():  # warm-up of every shape
@@ -101,9 +106,12 @@ def main():
                 fod_finite = all(np.isfinite(i["d4n_dfreq4"]).all() for i in infos)
                 b4 = np.array([i["beta4"] for i in infos])
                 res_fod = np.array([i["d4n_residual"] for i in infos])
+            if k == "disp_eps":
+                dmap_finite = all(np.isfinite(i["d2n_dfreq2_deps"]).all() for i in infos)
             if k == "fd3":
                 _, _, ng["fd3"], disp["fd3"] = plugin.group_index(np.array([o[1] for o in out]), f3, a.step)
-    nsolve = {"plain": a.nf, "analytic": a.nf, "analytic_gvd": a.nf, "gvd_eps": a.nf, "group_eps": a.nf, "analytic_tod": a.nf, "analytic_fod": a.nf, "fd3": 3 * a.nf}
+    nsolve = {"plain": a.nf, "analytic": a.nf, "analytic_gvd": a.nf, "gvd_eps": a.nf, "group_eps": a.nf, "analytic_tod": a.nf, "analytic_fod": a.nf, "fod_group_eps": a.nf, "disp_eps": a.nf,
+              "fd3": 3 * a.nf}
     N, M = a.n * a.n, wl.mode_spec.num_modes
     # one derivative pass reads, per (problem, mode), the real fp64 Ritz vector (2N x 8 B) and the three coefficient fields
     # (exx, eyy, 1/ezz: 3N x 8 B; shared by the sweep, counted once per mode pass as they are re-read)
@@ -113,6 +121,7 @@ def main():
     gmap_ms = (np.median(dev["group_eps"]) - np.median(dev["gvd_eps"]))
     tod_ms = (np.median(dev["analytic_tod"]) - np.median(dev["analytic_gvd"]))
     fod_ms = (np.median(dev["analytic_fod"]) - np.median(dev["analytic_tod"]))
+    dmap_ms = (np.median(dev["disp_eps"]) - np.median(dev["fod_group_eps"]))
     # the eigen-solves of the two arms are bit-identical, so the difference of the summed inner iterations is the correction
     # solves' (per problem: the slowest problem of its device batch, as for the eigen-solve's own counters)
     corr_iters = (np.median(inner["analytic_gvd"]) - np.median(inner["analytic"])) / (a.nf * M)
@@ -131,6 +140,7 @@ def main():
         beta3_range_ps3_per_km=[float(b3.min()), float(b3.max())],
         fourth_order_device_ms_per_problem=float(fod_ms / a.nf), fourth_order_finite=bool(fod_finite),
         beta4_range_ps4_per_km=[float(b4.min()), float(b4.max())],
+        dispersion_gradient_map_device_ms_per_problem=float(dmap_ms / a.nf), dispersion_gradient_map_finite=bool(dmap_finite),
         second_correction_inner_iters_per_mode=float(corr2_iters), second_correction_residual_max=float(res_fod.max()),
         correction_inner_iters_per_mode=float(corr_iters),
         correction_residual_max=float(res_gvd.max()),
