@@ -236,8 +236,8 @@ typedef struct {
                             rows xx / yy / zz are those of dn_deps bit for bit and the six off-diagonal rows are 0 -- the reference
                             solves such a problem as a diagonal one, and its n does not depend on off-diagonal components below
                             the tensorial threshold.  Not together with dn_deps on a tensorial problem (B200MS_ERR_ARG) */
-  int left_paired;       /* out: -1 when none of dn_dfreq, dn_deps, dn_deps_tensor, d2n_dfreq2, d2n_dfreq_deps, d3n_dfreq3 is asked
-                            for; else the number of modes whose left eigenvector is known: num_modes for diagonal problems (it
+  int left_paired;       /* out: -1 when none of dn_dfreq, dn_deps, dn_deps_tensor, d2n_dfreq2, d2n_dfreq_deps, d3n_dfreq3 (nor
+                            b200ms_pert.dn_dpert) is asked for; else the number of modes whose left eigenvector is known: num_modes for diagonal problems (it
                             follows from the structure of the operator), and for tensorial ones the modes whose transposed Ritz
                             value n_L was paired one-to-one with the mode's n (|n_L - n| <= 1e-6 |n|, both solves converged) and
                             whose unit left / right vectors w, u have |w^T u| >= 1e-8 */
@@ -282,6 +282,30 @@ typedef struct {
                               for a real change of eps: -1e18 f^2 (2 Re d2n_dfreq_deps + f Re d2n_dfreq2_deps) / c0^2 (c0 in um/s).
                               HOST or DEVICE memory like `fields` */
 } b200ms_result_ext2;
+
+/* ---- Response of each mode to caller-given permittivity perturbations (b200ms_solve_batch_ext3; the version stays 211).  The
+   permittivity gradients of dn_deps / dn_deps_tensor, d2n_dfreq_deps and d2n_dfreq2_deps contracted on the device against npert
+   fields delta eps_k (sum over every Yee site and component of map * delta eps_k), without writing or delivering the maps: the
+   same solves, and per-site forms summed against delta eps_k in a fixed order (deterministic, independent of batch position).
+   Perturbations are taken at fixed PML stretch, mu, d eps / df and d^2 eps / df^2.  Same scope as the map each output contracts;
+   n_complex, the fields and every other derivative and map do not change when it is asked for.  Indexed like prob / res. ---- */
+typedef struct {
+  int npert;                 /* K >= 1 when any output below is asked for */
+  const double *eps_pert;    /* NULL, or npert x 9 x nx x ny complex128 (re,im): delta eps_k in the layout of problem.eps; diagonal
+                                problems read components xx, yy, zz, tensorial ones (left_solve) all nine.  HOST or DEVICE memory.
+                                Only with problem.eps (else B200MS_ERR_ARG); problems that pass the same pointer share one copy */
+  const double *pert_table;  /* NULL, or npert x problem.section->nmedia x 9 complex128 (re,im): delta eps of each medium of the
+                                problem's section, rasterised like eps_table.  Only with problem.section (else B200MS_ERR_ARG) */
+  double *dn_dpert;          /* NULL, or caller-allocated npert x num_modes complex128 (re,im): d(n_eff + i k_eff) per unit amplitude
+                                of delta eps_k.  Needs eps_pert or pert_table (else B200MS_ERR_ARG).  Scope of dn_deps (tensorial
+                                problems: of dn_deps_tensor, with left_solve); NaN for an unpaired tensorial mode */
+  double *d2n_dfreq_dpert;   /* NULL, or npert x num_modes complex128: d(dn/df) (1/Hz) per unit amplitude of delta eps_k.  Needs
+                                dn_dpert and result.d2n_dfreq2 (else B200MS_ERR_ARG); scope of d2n_dfreq_deps; NaN where d2n_dfreq2 is.
+                                The group index responds by Re dn_dpert + f Re d2n_dfreq_dpert, also for a complex delta eps */
+  double *d2n_dfreq2_dpert;  /* NULL, or npert x num_modes complex128: d(d^2n/df^2) (1/Hz^2) per unit amplitude of delta eps_k.
+                                Needs d2n_dfreq_dpert and b200ms_result_ext.d4n_dfreq4 (else B200MS_ERR_ARG); scope of
+                                d2n_dfreq2_deps; NaN where d4n_dfreq4 is */
+} b200ms_pert;
 
 /* Tunables (all have defaults; see DESIGN.md). */
 typedef struct {
@@ -391,6 +415,10 @@ int b200ms_solve_batch_ext(b200ms_handle *h, int nprob, const b200ms_problem *pr
  * rext2 NULL). */
 int b200ms_solve_batch_ext2(b200ms_handle *h, int nprob, const b200ms_problem *prob, b200ms_result *res, const b200ms_problem_ext *pext,
                             const b200ms_result_ext *rext, const b200ms_result_ext2 *rext2);
+/* b200ms_solve_batch_ext2 with the perturbation responses: pert is NULL or nprob entries (b200ms_solve_batch_ext2 is this call
+ * with pert NULL). */
+int b200ms_solve_batch_ext3(b200ms_handle *h, int nprob, const b200ms_problem *prob, b200ms_result *res, const b200ms_problem_ext *pext,
+                            const b200ms_result_ext *rext, const b200ms_result_ext2 *rext2, const b200ms_pert *pert);
 
 /* Benchmark / roofline hook: run one of the two hot stencil kernels `nrep` times on `nbatch` device-resident copies
  * of the operator of `prob` and return the mean kernel time (CUDA events on the library stream).

@@ -65,6 +65,11 @@ class ResultExt2(C.Structure):
     _fields_ = [("d2n_dfreq2_deps", _dp)]
 
 
+class Pert(C.Structure):
+    _fields_ = [("npert", C.c_int), ("eps_pert", _dp), ("pert_table", _dp), ("dn_dpert", _dp), ("d2n_dfreq_dpert", _dp),
+                ("d2n_dfreq2_dpert", _dp)]
+
+
 class Options(C.Structure):
     _fields_ = [
         ("eig_tol", C.c_double), ("inner_tol", C.c_double), ("ncv", C.c_int), ("max_restarts", C.c_int),
@@ -85,7 +90,7 @@ class Stats(C.Structure):
 
 EXPORTS = [
     "b200ms_version", "b200ms_get_stats", "b200ms_default_options", "b200ms_create", "b200ms_destroy", "b200ms_set_options",
-    "b200ms_last_error", "b200ms_host_alloc", "b200ms_host_free", "b200ms_solve_batch", "b200ms_solve_batch_ext", "b200ms_solve_batch_ext2", "b200ms_bench_stencil", "b200ms_debug_schur", "b200ms_debug_setup",
+    "b200ms_last_error", "b200ms_host_alloc", "b200ms_host_free", "b200ms_solve_batch", "b200ms_solve_batch_ext", "b200ms_solve_batch_ext2", "b200ms_solve_batch_ext3", "b200ms_bench_stencil", "b200ms_debug_schur", "b200ms_debug_setup",
     "b200ms_debug_hierarchy", "b200ms_debug_batch", "b200ms_debug_apply", "b200ms_debug_vcycle", "b200ms_debug_solve", "b200ms_debug_march2_geometry", "b200ms_debug_post_tables", "b200ms_debug_post_tables_bounded", "b200ms_debug_te_terms", "b200ms_debug_grid_factors", "b200ms_debug_krylov", "b200ms_debug_fields",
 ]  # fmt: skip
 
@@ -127,6 +132,8 @@ def lib():
                                                  C.POINTER(ResultExt)]
             L.b200ms_solve_batch_ext2.argtypes = [C.c_void_p, C.c_int, C.POINTER(Problem), C.POINTER(Result), C.POINTER(ProblemExt),
                                                   C.POINTER(ResultExt), C.POINTER(ResultExt2)]
+            L.b200ms_solve_batch_ext3.argtypes = [C.c_void_p, C.c_int, C.POINTER(Problem), C.POINTER(Result), C.POINTER(ProblemExt),
+                                                  C.POINTER(ResultExt), C.POINTER(ResultExt2), C.POINTER(Pert)]
             L.b200ms_bench_stencil.argtypes = [C.c_void_p, C.POINTER(Problem), C.c_int, C.c_int, C.c_int, C.c_int, _dp, _dp, _dp, _dp]
             L.b200ms_debug_schur.argtypes = [C.c_int, _dp, _dp, _dp]
             L.b200ms_debug_setup.argtypes = [C.POINTER(Problem), _dp, _ip, _dp, _dp, _dp, _dp, _dp]
@@ -156,7 +163,7 @@ class PackedProblem:
     def __init__(self, eps_cross, coords, freq, mode_spec, symmetry=(0, 0), direction="+", eps_packed=None, basis_fields=None,
                  mu_cross=None, target_override=None, incidence=False, post=0, section=None, grid_correction=None, plane_bounds=None,
                  eps_dfreq=None, derivatives=False, eps_d2freq=None, second=False, eps_d3freq=None, third=False, left_solve=False, eps_d4freq=None,
-                 fourth=False):
+                 fourth=False, eps_pert=None, eps_pert_packed=None):
         self.section = None
         if section is not None:  # geometric cross-section rasterised on the device (tidy3d_b200/sections.py); no eps array
             self.section, self._section_arrays = section.pack(float(freq), (len(coords[0]) - 1, len(coords[1]) - 1), dispersion=derivatives,
@@ -288,8 +295,33 @@ class PackedProblem:
             self.d4eps_table = section.d4_table(float(freq))
             if self.d4eps_table is not None:
                 self.ext.d4eps_table = _ptr(self.d4eps_table.view(np.float64))
+        self.pert = Pert()  # the perturbation fields (b200ms_pert); outputs are attached by Handle.solve_batch
+        self.eps_pert = self.pert_table = None
+        if eps_pert is not None:
+            if section is not None:  # K dicts {Medium: change of its eps}, rasterised on the device like eps_table
+                self.pert_table = section.pert_table(eps_pert)
+                self.pert.npert = self.pert_table.shape[0]
+                self.pert.pert_table = _ptr(self.pert_table.view(np.float64))
+            else:
+                # an array packed for an earlier problem of the call is reused only on the same grid; else it is packed (and checked) anew
+                shared = eps_pert_packed is not None and eps_pert_packed.shape[1:] == (9, self.nx, self.ny)
+                self.eps_pert = eps_pert_packed if shared else pack_eps_pert(eps_pert, self.nx, self.ny)
+                self.pert.npert = self.eps_pert.shape[0]
+                self.pert.eps_pert = _ptr(self.eps_pert.view(np.float64))
         self.struct = p
         self.num_modes = p.num_modes
+
+
+def pack_eps_pert(eps_pert, nx, ny):
+    """(K, 9, nx, ny) contiguous complex128 perturbation fields of an eps_cross problem ((9, nx, ny): K = 1)."""
+    if isinstance(eps_pert, dict) or (isinstance(eps_pert, (list, tuple)) and eps_pert and isinstance(eps_pert[0], dict)):
+        raise ValueError("eps_pert: per-medium dicts need a 'section'; an eps_cross problem takes a (K, 9, Nx, Ny) array")
+    a = np.asarray(eps_pert, dtype=np.complex128)
+    if a.ndim == 3:
+        a = a[None]
+    if a.ndim != 4 or a.shape[0] < 1 or a.shape[1:] != (9, nx, ny):
+        raise ValueError(f"eps_pert must have shape (K, 9, {nx}, {ny}) or (9, {nx}, {ny}) (the layout of eps_cross), got {np.shape(eps_pert)}")
+    return np.ascontiguousarray(a)
 
 
 class PinnedPool:
@@ -380,7 +412,7 @@ class Handle:
 
     def solve_batch(self, packed, want_fields=True, fields_ptrs=None, want_flux=False, want_overlaps=False, want_dfreq=False, want_deps=False,
                     want_d2freq=False, want_group_eps=False, want_d3freq=False, want_deps_tensor=False, want_d4freq=False,
-                    want_d2freq2_deps=False):
+                    want_d2freq2_deps=False, want_pert=False, want_group_pert=False, want_disp_pert=False):
         """packed: list of PackedProblem.  Returns (rc, fields list | None, n_complex list, Result structs).
 
         ``fields_ptrs``: optional list of raw addresses (host or DEVICE memory, e.g. ``tensor.data_ptr()``) the library
@@ -393,13 +425,21 @@ class Handle:
         (9, nx, ny, M) arrays in ``last_dn_deps``; not together with ``want_deps``); ``want_d4freq``: d^4 n / df^4 of every mode and the
         residual of its second correction solve (``last_d4n_dfreq4`` / ``last_d4n_residual``, b200ms_solve_batch_ext; needs
         ``want_d3freq``); ``want_d2freq2_deps``: d(d^2n/df^2) / d eps of every mode from the corrections of both passes
-        (``last_d2n_dfreq2_deps``, b200ms_solve_batch_ext2; needs ``want_group_eps`` and ``want_d4freq``)."""
+        (``last_d2n_dfreq2_deps``, b200ms_solve_batch_ext2; needs ``want_group_eps`` and ``want_d4freq``); ``want_pert``: d n per unit
+        amplitude of each problem's perturbation fields (``last_dn_dpert``, (K, M) arrays, None for a problem without them;
+        b200ms_solve_batch_ext3); ``want_group_pert``: d(dn/df) of the same (``last_d2n_dfreq_dpert``; needs ``want_pert`` and
+        ``want_d2freq``); ``want_disp_pert``: d(d^2n/df^2) of the same (``last_d2n_dfreq2_dpert``; needs ``want_group_pert`` and
+        ``want_d4freq``)."""
         if want_deps and want_deps_tensor:
             raise ValueError("want_deps and want_deps_tensor fill the same list: ask for one of them")
         if want_d4freq and not want_d3freq:
             raise ValueError("want_d4freq needs want_d3freq: the fourth derivative is formed from the third-order pass")
         if want_d2freq2_deps and not (want_group_eps and want_d4freq):
             raise ValueError("want_d2freq2_deps needs want_group_eps and want_d4freq: the map is formed from both passes' corrections")
+        if want_group_pert and not (want_pert and want_d2freq):
+            raise ValueError("want_group_pert needs want_pert and want_d2freq")
+        if want_disp_pert and not (want_group_pert and want_d4freq):
+            raise ValueError("want_disp_pert needs want_group_pert and want_d4freq")
         n = len(packed)
         probs = (Problem * n)(*[p.struct for p in packed])
         results = (Result * n)()
@@ -409,6 +449,8 @@ class Handle:
         self.last_d4n_dfreq4, self.last_d4n_residual, self.last_d2n_dfreq2_deps = [], [], []
         rext = (ResultExt * n)() if want_d4freq else None
         rext2 = (ResultExt2 * n)() if want_d2freq2_deps else None
+        pert = (Pert * n)(*[p.pert for p in packed]) if want_pert else None
+        self.last_dn_dpert, self.last_d2n_dfreq_dpert, self.last_d2n_dfreq2_dpert = [], [], []
         for i, p in enumerate(packed):
             nc = np.zeros(p.num_modes, dtype=np.complex128)
             ncs.append(nc)
@@ -449,6 +491,13 @@ class Handle:
                 d = np.zeros((3, p.nx, p.ny, p.num_modes), dtype=np.complex128)
                 self.last_d2n_dfreq2_deps.append(d)
                 rext2[i].d2n_dfreq2_deps = _ptr(d.view(np.float64))
+            for want, last, name in ((want_pert, self.last_dn_dpert, "dn_dpert"), (want_group_pert, self.last_d2n_dfreq_dpert, "d2n_dfreq_dpert"),
+                                     (want_disp_pert, self.last_d2n_dfreq2_dpert, "d2n_dfreq2_dpert")):
+                if want:
+                    d = np.zeros((p.pert.npert, p.num_modes), dtype=np.complex128) if p.pert.npert else None
+                    last.append(d)
+                    if d is not None:
+                        setattr(pert[i], name, _ptr(d.view(np.float64)))
             if want_flux:
                 fl, te = np.zeros(p.num_modes), np.zeros(p.num_modes)
                 self.last_flux.append(fl)
@@ -468,7 +517,10 @@ class Handle:
                 results[i].fields = C.cast(C.c_void_p(f.ctypes.data), _dp)
             else:
                 results[i].fields = None
-        if want_d4freq:
+        if want_pert:
+            pext = (ProblemExt * n)(*[p.ext for p in packed])
+            rc = lib().b200ms_solve_batch_ext3(self._h, n, probs, results, pext, rext, rext2, pert)
+        elif want_d4freq:
             pext = (ProblemExt * n)(*[p.ext for p in packed])
             if want_d2freq2_deps:
                 rc = lib().b200ms_solve_batch_ext2(self._h, n, probs, results, pext, rext, rext2)

@@ -63,6 +63,7 @@ struct b200ms_handle {
   DevBuf post;        // interpolation tables / partials / results of the on-device post-processing
   DevBuf deriv;       // tables, partial sums, dispersion input and d n / d eps map of the derivative pass
   DevBuf disp;        // tables, material directions and partial sums of the dispersion pass
+  DevBuf pert_dev;    // perturbation fields of a device batch and the partial sums of their contraction (b200ms_pert)
   DevBuf warm;        // sorted Ritz vectors of the previous device batch of this call ([k][B][len]): warm start of the next one
   int warm_B = 0, warm_k = 0, warm_tsize = 0;
   size_t warm_len = 0;
@@ -77,6 +78,7 @@ struct b200ms_handle {
   const b200ms_problem_ext *pext = nullptr;  // the fourth-order arrays of the b200ms_solve_batch_ext call in progress, or null
   const b200ms_result_ext *rext = nullptr;
   const b200ms_result_ext2 *rext2 = nullptr;  // the dispersion-gradient maps of a b200ms_solve_batch_ext2 call in progress, or null
+  const b200ms_pert *pert = nullptr;          // the perturbation responses of a b200ms_solve_batch_ext3 call in progress, or null
 };
 
 extern "C" int b200ms_version(void) { return B200MS_VERSION; }
@@ -161,6 +163,7 @@ extern "C" int b200ms_destroy(b200ms_handle *h) {
   h->warm.release();
   h->deriv.release();
   h->disp.release();
+  h->pert_dev.release();
   if (h->io_stream) cudaStreamDestroy(h->io_stream);
   if (h->dl_stream) cudaStreamDestroy(h->dl_stream);
   if (h->flush_buf) cudaFree(h->flush_buf);
@@ -232,6 +235,9 @@ inline size_t align256(size_t n) { return (n + 255) & ~size_t(255); }
 inline bool asks_derivatives(const b200ms_result &r) {
   return r.dn_dfreq || r.dn_deps || r.dn_deps_tensor || r.d2n_dfreq2 || r.d2n_dfreq_deps || r.d3n_dfreq3;
 }
+
+// the perturbation responses problem i of the call in progress asks for, or null (every output needs dn_dpert)
+inline const b200ms_pert *pert_of(const b200ms_handle *h, int i) { return (h->pert && h->pert[i].dn_dpert) ? h->pert + i : nullptr; }
 
 // A window of consecutive problems whose raw media are resident on the device: set-up stages A-C of host_setup.hpp with
 // the per-cell work (reductions) done by medium_scan_kernel.
@@ -762,12 +768,168 @@ size_t gather_scratch_bytes(const std::vector<int> &ids, const Window &W, const 
   return bytes;
 }
 
+// The perturbations (b200ms_pert) of a device batch on the device, in h->pert_dev: perturbation k0 + j of problem b at
+// eps + j kstride + b bstride ([ncomp][N]; zero for a problem that asks for none or has fewer), kg of them at a time, then the
+// partial and reduced sums of the contraction kernels.
+struct PertSet {
+  int K = 0;             // the largest npert of the batch's problems (0: no problem asks)
+  int kg = 0, k0 = -1;   // perturbations held at once, and the first one held (-1: none yet)
+  int ncomp = 3;
+  bool shared = false;   // every problem passes the same eps_pert: one copy, batch stride 0
+  cplx *eps = nullptr;
+  size_t kstride = 0, bstride = 0;
+  cplx *partial = nullptr, *sums = nullptr;
+  unsigned char *scratch = nullptr;  // gather_diag's section scratch
+};
+
+// Perturbations held on the device at once (a device group): at most kPertHeld, and at most what fits in an eighth of the free
+// device memory (at least one), so that the buffer leaves room for the dispersion pass's scratch, which is reserved after it.
+// Past that the perturbations are gathered again group by group (per mode slot in the dispersion pass); which perturbations
+// share a device group changes no bit of any sum.
+constexpr int kPertHeld = 16;
+
+// Sizes h->pert_dev for the batch (ncomp 3: diagonal, 9: tensorial).
+PertSet pert_setup(b200ms_handle *h, const std::vector<int> &ids, const Window &W, const b200ms_problem *prob, int nx, int ny, int k,
+                   int ncomp) {
+  PertSet P;
+  const int B = (int)ids.size();
+  const size_t N = (size_t)nx * ny;
+  const b200ms_pert *first = nullptr;
+  P.shared = true;
+  for (int b = 0; b < B; ++b) {
+    const b200ms_pert *q = pert_of(h, W.i0 + ids[b]);
+    if (q) P.K = std::max(P.K, q->npert);
+    if (!q || !q->eps_pert || (first && (q->eps_pert != first->eps_pert || q->npert != first->npert))) P.shared = false;
+    if (q && !first) first = q;
+  }
+  if (P.K == 0) return P;
+  P.ncomp = ncomp;
+  const int Bc = P.shared ? 1 : B;
+  const size_t per = align256((size_t)Bc * ncomp * N * sizeof(cplx));
+  size_t free_b = 0, total_b = 0;
+  CUDA_CHECK(cudaMemGetInfo(&free_b, &total_b));
+  P.kg = (int)std::max<size_t>(1, std::min<size_t>(std::min(P.K, kPertHeld), (free_b + h->pert_dev.cap) / 8 / per));
+  P.bstride = P.shared ? 0 : ncomp * N;
+  P.kstride = per / sizeof(cplx);
+  const int nch = (int)std::min<size_t>(kDerivChunks, (N + 255) / 256);
+  const size_t nblk = (size_t)((ny + 63) / 64) * ((nx + 3) / 4);
+  const size_t npart = std::max((size_t)B * k * kPertGroup * nch, (size_t)B * P.kg * 3 * nblk);  // scans; per-site kernels (NF <= 3)
+  const size_t nsum = std::max((size_t)B * k * kPertGroup, (size_t)B * P.kg * 3);
+  auto tab0 = [h, prob](const b200ms_problem &p) {
+    const b200ms_pert *q = pert_of(h, (int)(&p - prob));
+    return q ? q->pert_table : nullptr;
+  };
+  const size_t sec = gather_scratch_bytes(ids, W, prob, nx, ny, tab0);
+  const size_t o_part = per * P.kg, o_sum = o_part + align256(npart * sizeof(cplx)), o_sec = o_sum + align256(nsum * sizeof(cplx));
+  h->pert_dev.reserve(o_sec + sec + 256);
+  P.eps = reinterpret_cast<cplx *>(h->pert_dev.p);
+  P.partial = reinterpret_cast<cplx *>(h->pert_dev.p + o_part);
+  P.sums = reinterpret_cast<cplx *>(h->pert_dev.p + o_sum);
+  P.scratch = h->pert_dev.p + o_sec;
+  return P;
+}
+
+// Holds perturbations k0 .. k0 + kg - 1 of the batch in P (no-op when they are already held); returns how many there are.
+int pert_load(b200ms_handle *h, PertSet &P, const std::vector<int> &ids, const Window &W, const b200ms_problem *prob, int nx, int ny, int k0) {
+  const int n = std::min(P.kg, P.K - k0);
+  if (P.k0 == k0) return n;
+  const size_t N = (size_t)nx * ny;
+  const std::vector<int> one(1, ids[0]);
+  for (int j = 0; j < n; ++j) {
+    const int kk = k0 + j;
+    auto arr = [h, prob, kk, N](const b200ms_problem &p) -> const double * {
+      const b200ms_pert *q = pert_of(h, (int)(&p - prob));
+      return (q && q->eps_pert && kk < q->npert) ? q->eps_pert + (size_t)kk * 9 * N * 2 : nullptr;
+    };
+    auto tab = [h, prob, kk](const b200ms_problem &p) -> const double * {
+      const b200ms_pert *q = pert_of(h, (int)(&p - prob));
+      return (q && q->pert_table && kk < q->npert) ? q->pert_table + (size_t)kk * p.section->nmedia * 9 * 2 : nullptr;
+    };
+    gather_diag(h, P.shared ? one : ids, W, prob, nx, ny, arr, tab, P.eps + j * P.kstride, P.scratch, P.ncomp);
+  }
+  P.k0 = k0;
+  return n;
+}
+
+// First-order responses of a batch after its scan (deriv_pert_kernel / tensor_pert_kernel launched by `launch` for each group of
+// at most kPertGroup perturbations): dn_dpert[k][q] = scale[b][q] * (sum of the gradient against delta eps_k).
+template <typename Launch>
+void pert_first_order(b200ms_handle *h, PertSet &P, const std::vector<int> &ids, const Window &W, const b200ms_problem *prob, int nx, int ny,
+                      int k, const std::vector<cplx> &scale, Launch launch) {
+  const int B = (int)ids.size();
+  const int nch = (int)std::min<size_t>(kDerivChunks, ((size_t)nx * ny + 255) / 256);
+  cudaStream_t st = h->stream;
+  NvtxRange r("b200ms:perturbation responses (first order)");
+  for (int g0 = 0; g0 < P.K; g0 += P.kg) {
+    const int ng = pert_load(h, P, ids, W, prob, nx, ny, g0);
+    for (int c0 = 0; c0 < ng; c0 += kPertGroup) {
+      const PertArgs pa{P.eps + c0 * P.kstride, P.kstride, P.bstride, std::min(kPertGroup, ng - c0), P.partial};
+      launch(pa);
+      deriv_final_kernel<<<(B * k * kPertGroup + 127) / 128, 128, 0, st>>>(P.partial, nch, B * k * kPertGroup, P.sums);
+      CUDA_CHECK(cudaGetLastError());
+      h->stats.launches += 2;
+      std::vector<cplx> s((size_t)B * k * kPertGroup);
+      CUDA_CHECK(cudaMemcpyAsync(s.data(), P.sums, s.size() * sizeof(cplx), cudaMemcpyDeviceToHost, st));
+      CUDA_CHECK(cudaStreamSynchronize(st));
+      for (int b = 0; b < B; ++b) {
+        const b200ms_pert *q = pert_of(h, W.i0 + ids[b]);
+        for (int c = 0; c < pa.npert && q; ++c) {
+          const int kk = g0 + c0 + c;
+          if (kk >= q->npert) break;
+          for (int m = 0; m < k; ++m) {
+            const cplx &v = s[((size_t)b * k + m) * kPertGroup + c], &sc = scale[(size_t)b * k + m];
+            const cd d = cd(sc.re, sc.im) * cd(v.re, v.im);
+            q->dn_dpert[2 * ((size_t)kk * k + m)] = d.real();
+            q->dn_dpert[2 * ((size_t)kk * k + m) + 1] = d.imag();
+          }
+        }
+      }
+    }
+  }
+}
+
+// Second-order responses of mode slot q (group_grad_kernel / disp_grad_kernel with PERT, launched by `launch` for each device
+// group): NF forms per perturbation, out[k][q] = sum_v coef[b][v] * (sum of form v against delta eps_k).  `out(b)` is the
+// problem's npert x num_modes output or null.
+template <int NF, typename Launch, typename Out>
+void pert_second_order(b200ms_handle *h, PertSet &P, const std::vector<int> &ids, const Window &W, const b200ms_problem *prob, int nx, int ny,
+                       int k, int q, const std::vector<cd> &coef, Launch launch, Out out) {
+  const int B = (int)ids.size();
+  const int nblk = ((ny + 63) / 64) * ((nx + 3) / 4);
+  cudaStream_t st = h->stream;
+  for (int g0 = 0; g0 < P.K; g0 += P.kg) {
+    const int ng = pert_load(h, P, ids, W, prob, nx, ny, g0), rows = (NF * ng + 2) / 3;
+    launch(PertArgs{P.eps, P.kstride, P.bstride, ng, P.partial});
+    deriv_final_kernel<<<(B * rows * 3 + 127) / 128, 128, 0, st>>>(P.partial, nblk, B * rows * 3, P.sums);
+    CUDA_CHECK(cudaGetLastError());
+    h->stats.launches += 2;
+    std::vector<cplx> s((size_t)B * rows * 3);
+    CUDA_CHECK(cudaMemcpyAsync(s.data(), P.sums, s.size() * sizeof(cplx), cudaMemcpyDeviceToHost, st));
+    CUDA_CHECK(cudaStreamSynchronize(st));
+    for (int b = 0; b < B; ++b) {
+      const b200ms_pert *pq = pert_of(h, W.i0 + ids[b]);
+      double *o = out(b);
+      if (!o) continue;
+      for (int c = 0; c < ng && g0 + c < pq->npert; ++c) {
+        cd d = 0.0;
+        for (int v = 0; v < NF; ++v) {
+          const cplx &z = s[(size_t)b * rows * 3 + NF * c + v];
+          d += coef[(size_t)b * NF + v] * cd(z.re, z.im);
+        }
+        o[2 * ((size_t)(g0 + c) * k + q)] = d.real();
+        o[2 * ((size_t)(g0 + c) * k + q) + 1] = d.imag();
+      }
+    }
+  }
+}
+
 // Derivative pass of one device batch (csrc/derivatives.cuh) on the sorted Ritz vectors: result.dn_dfreq and result.dn_deps of
 // the problems that ask for them.  Reads only; the eigenpairs and fields of the batch are those of a run without it.  `out`
 // receives the pass's device tables (valid until h->deriv is reserved again) for the dispersion pass.
 template <typename T, typename C, typename P, typename PC>
 void derivative_pass(b200ms_handle *h, BatchSolver<T, C, P, PC> &S, const std::vector<const ProblemSetup *> &ps, const std::vector<int> &ids,
-                     const Window &W, const b200ms_problem *prob, b200ms_result *res, const std::vector<cd> &nsorted, DerivArgs<T, C> &out) {
+                     const Window &W, const b200ms_problem *prob, b200ms_result *res, const std::vector<cd> &nsorted, DerivArgs<T, C> &out,
+                     PertSet &pset) {
   const int B = (int)ids.size(), k = S.k, nx = S.nx, ny = S.ny;
   const size_t N = (size_t)nx * ny;
   bool any_map = false, any_disp = false;
@@ -863,6 +1025,11 @@ void derivative_pass(b200ms_handle *h, BatchSolver<T, C, P, PC> &S, const std::v
       }
     }
   }
+  if (pset.K)
+    pert_first_order(h, pset, ids, W, prob, nx, ny, k, scale, [&](const PertArgs &pa) {
+      if (S.has_mu) deriv_pert_kernel<T, C, true><<<dim3(nch, B * k), 256, 0, st>>>(a, pa);
+      else deriv_pert_kernel<T, C, false><<<dim3(nch, B * k), 256, 0, st>>>(a, pa);
+    });
   if (!any_map) return;
   CUDA_CHECK(cudaMemcpyAsync(base + o_scale, scale.data(), scale.size() * sizeof(cplx), cudaMemcpyHostToDevice, st));
   dim3 blk(64, 4), grd((ny + 63) / 64, (nx + 3) / 4, B * k);
@@ -939,7 +1106,7 @@ std::vector<char> left_vectors(b200ms_handle *h, BatchSolver<T, C, P, PC> &S, co
 template <typename T, typename C, typename P, typename PC>
 void tensor_derivative_pass(b200ms_handle *h, BatchSolver<T, C, P, PC> &S, const std::vector<const ProblemSetup *> &ps, const std::vector<int> &ids,
                             const Window &W, const b200ms_problem *prob, b200ms_result *res, const std::vector<char> &paired,
-                            const MediumRef *d_refs, bool share) {
+                            const MediumRef *d_refs, bool share, PertSet &pset) {
   if constexpr (std::is_same<T, cplx>::value) {
     const int B = (int)ids.size(), k = S.k, nx = S.nx, ny = S.ny;
     const size_t N = (size_t)nx * ny;
@@ -1032,6 +1199,9 @@ void tensor_derivative_pass(b200ms_handle *h, BatchSolver<T, C, P, PC> &S, const
       r.left_paired = np;
     }
     if (h->opt.verbose) fprintf(stderr, "[b200ms] transposed solve: smallest paired |w^T u| %.2e\n", smallest);
+    if (pset.K)
+      pert_first_order(h, pset, ids, W, prob, nx, ny, k, scale,
+                       [&](const PertArgs &pa) { tensor_pert_kernel<C><<<dim3(nch, B * k), 256, 0, st>>>(a, pa); });
     if (!any_map) return;
     CUDA_CHECK(cudaMemcpyAsync(base + o_scale, scale.data(), scale.size() * sizeof(cplx), cudaMemcpyHostToDevice, st));
     tensor_deriv_map_kernel<C><<<dim3((ny + 63) / 64, (nx + 3) / 4, B * k), dim3(64, 4), 0, st>>>(a);
@@ -1057,15 +1227,16 @@ void tensor_derivative_pass(b200ms_handle *h, BatchSolver<T, C, P, PC> &S, const
 // sums the products of lambda''''.  With b200ms_result_ext2.d2n_dfreq2_deps (which needs d2n_dfreq_deps and d4n_dfreq4),
 // disp_grad_kernel then writes slot q of the map d_g (d^2n/df^2) from the same x and x2.  It writes its own buffers, the
 // first four slots of the outer Krylov basis and the inner solver's scratch -- nothing the fields, the post-processing or the
-// warm start read.
+// warm start read.  b200ms_pert.d2n_dfreq_dpert / d2n_dfreq2_dpert run the PERT instantiations of the same two kernels at the
+// same points (pert_second_order), in place of or beside the maps.
 template <typename T, typename C, typename P, typename PC>
 void dispersion_pass(b200ms_handle *h, BatchSolver<T, C, P, PC> &S, const std::vector<const ProblemSetup *> &ps, const std::vector<int> &ids,
                      const Window &W, const b200ms_problem *prob, b200ms_result *res, const std::vector<cd> &nsorted,
-                     const std::vector<cd> &lam, const DerivArgs<T, C> &da) {
+                     const std::vector<cd> &lam, const DerivArgs<T, C> &da, PertSet &pset) {
   const int B = (int)ids.size(), k = S.k, nx = S.nx, ny = S.ny;
   const size_t N = (size_t)nx * ny;
   std::vector<char> skip(B), skip4(B, 1);
-  bool any_mat = false, any_gmap = false, any_third = false, any_fourth = false, any_dgrad = false;
+  bool any_mat = false, any_gmap = false, any_third = false, any_fourth = false, any_dgrad = false, any_gpert = false, any_dpert = false;
   for (int b = 0; b < B; ++b) {
     const b200ms_problem &p = prob[W.i0 + ids[b]];
     const b200ms_result &rb = res[W.i0 + ids[b]];
@@ -1075,6 +1246,9 @@ void dispersion_pass(b200ms_handle *h, BatchSolver<T, C, P, PC> &S, const std::v
     skip4[b] = (h->rext && h->rext[W.i0 + ids[b]].d4n_dfreq4) ? 0 : 1;
     any_fourth = any_fourth || !skip4[b];
     any_dgrad = any_dgrad || (h->rext2 && h->rext2[W.i0 + ids[b]].d2n_dfreq2_deps);
+    const b200ms_pert *pq = pert_of(h, W.i0 + ids[b]);
+    any_gpert = any_gpert || (pq && pq->d2n_dfreq_dpert);
+    any_dpert = any_dpert || (pq && pq->d2n_dfreq2_dpert);
     any_mat = any_mat || (p.eps ? (p.eps_dfreq || p.eps_d2freq) : (p.section->deps_table || p.section->d2eps_table));
   }
   for (int b = 0; b < B && any_third; ++b) {  // the third-order terms also read eps'''
@@ -1150,7 +1324,7 @@ void dispersion_pass(b200ms_handle *h, BatchSolver<T, C, P, PC> &S, const std::v
   // group-gradient pass: per-problem (alpha, beta), the sum w_hat^T v and the map [B][3][N][M]
   const size_t o_ab = align256(o_sec + sec_bytes), o_hsum = o_ab + align256((size_t)B * 2 * sizeof(cplx));
   const size_t o_gmap = o_hsum + align256((size_t)B * 3 * sizeof(cplx));
-  size_t end = any_gmap ? o_gmap + align256((size_t)B * 3 * N * k * sizeof(cplx)) : align256(o_sec + sec_bytes);
+  size_t end = any_gmap ? o_gmap + align256((size_t)B * 3 * N * k * sizeof(cplx)) : (any_gpert ? o_gmap : align256(o_sec + sec_bytes));
   // third-order pass: c''', c' + c'', c' - c'' per axis, p''', p' + p'', p' - p'', its partial sums and the six sums per problem
   size_t o_c3[6] = {0, 0, 0, 0, 0, 0}, o_p3 = 0, o_tpart = 0, o_tsum = 0;
   if (any_third) {
@@ -1184,11 +1358,11 @@ void dispersion_pass(b200ms_handle *h, BatchSolver<T, C, P, PC> &S, const std::v
   }
   // dispersion-gradient pass: (beta_0, beta_1, beta_2) per problem and the map [B][3][N][M]
   size_t o_dbeta = 0, o_dmap = 0;
-  if (any_dgrad) {
+  if (any_dgrad || any_dpert) {
     o_dbeta = end;
     end += align256((size_t)B * 3 * sizeof(cplx));
     o_dmap = end;
-    end += align256((size_t)B * 3 * N * k * sizeof(cplx));
+    if (any_dgrad) end += align256((size_t)B * 3 * N * k * sizeof(cplx));
   }
   h->disp.reserve(end + 256);
   unsigned char *base = h->disp.p;
@@ -1320,7 +1494,7 @@ void dispersion_pass(b200ms_handle *h, BatchSolver<T, C, P, PC> &S, const std::v
       rr.d2n_dfreq2[2 * q + 1] = d2n.imag();
       if (rr.d2n_residual) rr.d2n_residual[q] = resv[b];
     }
-    if (any_gmap) {  // d_g (dn/df) of slot q while x still holds its correction
+    if (any_gmap || any_gpert) {  // d_g (dn/df) of slot q while x still holds its correction
       const dim3 g0(nch, B);
       cplx *hsum = reinterpret_cast<cplx *>(base + o_hsum), *dab = reinterpret_cast<cplx *>(base + o_ab);
       cplx *gmap = reinterpret_cast<cplx *>(base + o_gmap);
@@ -1342,12 +1516,29 @@ void dispersion_pass(b200ms_handle *h, BatchSolver<T, C, P, PC> &S, const std::v
         ab[2 * b] = mk(al.real(), al.imag());
         ab[2 * b + 1] = mk(be.real(), be.imag());
       }
-      CUDA_CHECK(cudaMemcpyAsync(dab, ab.data(), ab.size() * sizeof(cplx), cudaMemcpyHostToDevice, st));
       const dim3 blk(64, 4), grd((ny + 63) / 64, (nx + 3) / 4, B);
-      if (S.has_mu) group_grad_kernel<T, C, true><<<grd, blk, 0, st>>>(a, 1, dab, gmap);
-      else group_grad_kernel<T, C, false><<<grd, blk, 0, st>>>(a, 1, dab, gmap);
-      CUDA_CHECK(cudaGetLastError());
-      h->stats.launches += 3;
+      h->stats.launches += 2;
+      if (any_gmap) {
+        CUDA_CHECK(cudaMemcpyAsync(dab, ab.data(), ab.size() * sizeof(cplx), cudaMemcpyHostToDevice, st));
+        if (S.has_mu) group_grad_kernel<T, C, true><<<grd, blk, 0, st>>>(a, 1, dab, gmap);
+        else group_grad_kernel<T, C, false><<<grd, blk, 0, st>>>(a, 1, dab, gmap);
+        CUDA_CHECK(cudaGetLastError());
+        h->stats.launches += 1;
+      }
+      if (any_gpert) {  // d(dn/df) = alpha sum (chi E + chi' D) . delta eps + beta sum chi D . delta eps
+        std::vector<cd> coef((size_t)B * 2);
+        for (size_t e = 0; e < coef.size(); ++e) coef[e] = cd(ab[e].re, ab[e].im);
+        pert_second_order<2>(
+            h, pset, ids, W, prob, nx, ny, k, q, coef,
+            [&](const PertArgs &pa) {
+              if (S.has_mu) group_grad_kernel<T, C, true, true><<<grd, blk, 0, st>>>(a, 1, dab, gmap, pa);
+              else group_grad_kernel<T, C, false, true><<<grd, blk, 0, st>>>(a, 1, dab, gmap, pa);
+            },
+            [&](int b) -> double * {
+              const b200ms_pert *pq = pert_of(h, W.i0 + ids[b]);
+              return pq ? pq->d2n_dfreq_dpert : nullptr;
+            });
+      }
     }
     if (any_third) {  // lambda''' of slot q from the same x (third_scan_kernel)
       const dim3 g0(nch, B);
@@ -1437,7 +1628,7 @@ void dispersion_pass(b200ms_handle *h, BatchSolver<T, C, P, PC> &S, const std::v
         re.d4n_dfreq4[2 * q + 1] = d4n.imag();
         if (re.d4n_residual) re.d4n_residual[q] = resv2[b];
       }
-      if (any_dgrad) {  // d_g (d^2n/df^2) of slot q while x and x2 still hold its corrections
+      if (any_dgrad || any_dpert) {  // d_g (d^2n/df^2) of slot q while x and x2 still hold its corrections
         std::vector<cplx> bg((size_t)B * 3);
         for (int b = 0; b < B; ++b) {
           const cplx *s = sv.data() + (size_t)b * 3, *t = sx.data() + (size_t)b * 3, *u = s3.data() + (size_t)b * 6, *z = s4.data() + (size_t)b * 12;
@@ -1455,12 +1646,28 @@ void dispersion_pass(b200ms_handle *h, BatchSolver<T, C, P, PC> &S, const std::v
           }
         }
         cplx *dbeta_g = reinterpret_cast<cplx *>(base + o_dbeta), *dmap = reinterpret_cast<cplx *>(base + o_dmap);
-        CUDA_CHECK(cudaMemcpyAsync(dbeta_g, bg.data(), bg.size() * sizeof(cplx), cudaMemcpyHostToDevice, st));
         const dim3 blk(64, 4), grd((ny + 63) / 64, (nx + 3) / 4, B);
-        if (S.has_mu) disp_grad_kernel<T, C, true><<<grd, blk, 0, st>>>(a, fa, dbeta_g, dmap);
-        else disp_grad_kernel<T, C, false><<<grd, blk, 0, st>>>(a, fa, dbeta_g, dmap);
-        CUDA_CHECK(cudaGetLastError());
-        h->stats.launches += 1;
+        if (any_dgrad) {
+          CUDA_CHECK(cudaMemcpyAsync(dbeta_g, bg.data(), bg.size() * sizeof(cplx), cudaMemcpyHostToDevice, st));
+          if (S.has_mu) disp_grad_kernel<T, C, true><<<grd, blk, 0, st>>>(a, fa, dbeta_g, dmap);
+          else disp_grad_kernel<T, C, false><<<grd, blk, 0, st>>>(a, fa, dbeta_g, dmap);
+          CUDA_CHECK(cudaGetLastError());
+          h->stats.launches += 1;
+        }
+        if (any_dpert) {  // d(d^2n/df^2) = sum_e beta_e sum E_e . delta eps
+          std::vector<cd> coef((size_t)B * 3);
+          for (size_t e = 0; e < coef.size(); ++e) coef[e] = cd(bg[e].re, bg[e].im);
+          pert_second_order<3>(
+              h, pset, ids, W, prob, nx, ny, k, q, coef,
+              [&](const PertArgs &pa) {
+                if (S.has_mu) disp_grad_kernel<T, C, true, true><<<grd, blk, 0, st>>>(a, fa, dbeta_g, dmap, pa);
+                else disp_grad_kernel<T, C, false, true><<<grd, blk, 0, st>>>(a, fa, dbeta_g, dmap, pa);
+              },
+              [&](int b) -> double * {
+                const b200ms_pert *pq = pert_of(h, W.i0 + ids[b]);
+                return pq ? pq->d2n_dfreq2_dpert : nullptr;
+              });
+        }
       }
     }
   }
@@ -1492,7 +1699,7 @@ void solve_group(b200ms_handle *h, const std::vector<int> &ids, const Window &W,
   bool left = false;
   for (int b = 0; b < B; ++b) {
     const b200ms_result &rb = res[W.i0 + ids[b]];
-    left = left || (ps[b]->tensorial && prob[W.i0 + ids[b]].left_solve && (rb.dn_dfreq || rb.dn_deps_tensor));
+    left = left || (ps[b]->tensorial && prob[W.i0 + ids[b]].left_solve && (rb.dn_dfreq || rb.dn_deps_tensor || pert_of(h, W.i0 + ids[b])));
   }
   S.pairing_ = left;
   const MediumRef *d_refs = upload_refs(h, refs, h->stream);
@@ -1586,16 +1793,18 @@ void solve_group(b200ms_handle *h, const std::vector<int> &ids, const Window &W,
   bool want_deriv = false, want_disp = false;
   for (int b = 0; b < B; ++b) {
     const b200ms_result &rb = res[W.i0 + ids[b]];
-    want_deriv = want_deriv || asks_derivatives(rb);
+    want_deriv = want_deriv || asks_derivatives(rb) || pert_of(h, W.i0 + ids[b]);
     want_disp = want_disp || rb.d2n_dfreq2 || rb.d2n_dfreq_deps || rb.d3n_dfreq3;
   }
   if (left) {
     const std::vector<char> paired = left_vectors(h, S, ps, nsorted, eig.nconv);
-    tensor_derivative_pass(h, S, ps, ids, W, prob, res, paired, d_refs, share);
+    PertSet pset = pert_setup(h, ids, W, prob, S.nx, S.ny, k, 9);
+    tensor_derivative_pass(h, S, ps, ids, W, prob, res, paired, d_refs, share, pset);
   } else if (want_deriv) {
     DerivArgs<T, C> da;
-    derivative_pass(h, S, ps, ids, W, prob, res, nsorted, da);
-    if (want_disp) dispersion_pass(h, S, ps, ids, W, prob, res, nsorted, lam, da);
+    PertSet pset = pert_setup(h, ids, W, prob, S.nx, S.ny, k, 3);
+    derivative_pass(h, S, ps, ids, W, prob, res, nsorted, da, pset);
+    if (want_disp) dispersion_pass(h, S, ps, ids, W, prob, res, nsorted, lam, da, pset);
   }
   CUDA_CHECK(cudaEventRecord(h->ev1, h->stream));
   CUDA_CHECK(cudaEventSynchronize(h->ev1));
@@ -1625,7 +1834,7 @@ void solve_group(b200ms_handle *h, const std::vector<int> &ids, const Window &W,
     r.op_applies = fwd.op_applies;
     r.inner_iters = fwd.inner_iters;
     r.stencil_applies = (int)std::min<long>(fwd.launches, 2147483647L);
-    if (!asks_derivatives(r)) r.left_paired = -1;
+    if (!asks_derivatives(r) && !pert_of(h, W.i0 + ids[b])) r.left_paired = -1;
     else if (!S.tensor_) r.left_paired = k;
     r.is_complex = real_arith ? 0 : 1;
     r.solve_ms = ms;
@@ -1679,7 +1888,8 @@ void dispatch_group(int kind, bool f32, A &&...a) {
 
 }  // namespace
 
-// The solve itself (b200ms_solve_batch_ext after its own checks; the fourth-order arrays are in h->pext / h->rext).
+// The solve itself (b200ms_solve_batch_ext3 after its own checks; the fourth-order arrays are in h->pext / h->rext, the
+// dispersion-gradient maps in h->rext2 and the perturbation responses in h->pert).
 static int solve_batch_impl(b200ms_handle *h, int nprob, const b200ms_problem *prob, b200ms_result *res) {
   if (cudaSetDevice(h->device) != cudaSuccess) return B200MS_ERR_CUDA;
   h->err.clear();
@@ -1736,7 +1946,7 @@ static int solve_batch_impl(b200ms_handle *h, int nprob, const b200ms_problem *p
           res[i].is_complex = s.is_complex;
           std::string err = s.error;
           const bool left = prob[i].left_solve != 0;
-          if (res[i].status == B200MS_OK && asks_derivatives(res[i]) && ((s.tensorial && !left) || s.relative || s.masked)) {
+          if (res[i].status == B200MS_OK && (asks_derivatives(res[i]) || pert_of(h, i)) && ((s.tensorial && !left) || s.relative || s.masked)) {
             res[i].status = B200MS_ERR_UNSUPPORTED;
             err = (s.tensorial && !left) ? "mode derivatives: tensorial problems (angled planes, off-diagonal eps) need the transposed eigen-solve: "
                                            "set b200ms_problem.left_solve (Python: left_solve=True), about one more eigen-solve"
@@ -1775,7 +1985,8 @@ static int solve_batch_impl(b200ms_handle *h, int nprob, const b200ms_problem *p
         for (auto &kv : groups) {
           const std::vector<int> &all = kv.second;
           bool left = false;
-          for (int id : all) left = left || (W.setups[id].tensorial && prob[i0 + id].left_solve && (res[i0 + id].dn_dfreq || res[i0 + id].dn_deps_tensor));
+          for (int id : all)
+            left = left || (W.setups[id].tensorial && prob[i0 + id].left_solve && (res[i0 + id].dn_dfreq || res[i0 + id].dn_deps_tensor || pert_of(h, i0 + id)));
           const size_t per = bytes_per_problem(W.setups[all[0]], h->opt, left);
           int bmax = (int)std::max<size_t>(1, std::min<size_t>((size_t)std::max(1, h->opt.max_batch), (size_t)(0.8 * free_b) / per));
           for (size_t s0 = 0; s0 < all.size();) {
@@ -1838,9 +2049,26 @@ static int solve_batch_impl(b200ms_handle *h, int nprob, const b200ms_problem *p
   return first_err;
 }
 
-extern "C" int b200ms_solve_batch_ext2(b200ms_handle *h, int nprob, const b200ms_problem *prob, b200ms_result *res,
-                                       const b200ms_problem_ext *pext, const b200ms_result_ext *rext, const b200ms_result_ext2 *rext2) {
+extern "C" int b200ms_solve_batch_ext3(b200ms_handle *h, int nprob, const b200ms_problem *prob, b200ms_result *res,
+                                       const b200ms_problem_ext *pext, const b200ms_result_ext *rext, const b200ms_result_ext2 *rext2,
+                                       const b200ms_pert *pert) {
   if (!h || nprob < 0 || (nprob > 0 && (!prob || !res))) return B200MS_ERR_ARG;
+  for (int i = 0; i < nprob && pert; ++i) {
+    const b200ms_pert &q = pert[i];
+    const char *why = nullptr;
+    if ((q.d2n_dfreq_dpert || q.d2n_dfreq2_dpert) && !q.dn_dpert) why = "d2n_dfreq_dpert and d2n_dfreq2_dpert need dn_dpert of the same problem";
+    else if (q.d2n_dfreq_dpert && !res[i].d2n_dfreq2) why = "d2n_dfreq_dpert needs d2n_dfreq2 of the same problem";
+    else if (q.d2n_dfreq2_dpert && !(q.d2n_dfreq_dpert && rext && rext[i].d4n_dfreq4))
+      why = "d2n_dfreq2_dpert needs d2n_dfreq_dpert and d4n_dfreq4 of the same problem";
+    else if (q.eps_pert && !prob[i].eps) why = "eps_pert belongs to an eps problem; a section's perturbations are given by pert_table";
+    else if (q.pert_table && prob[i].eps) why = "pert_table belongs to a section problem; an eps problem's perturbations are given by eps_pert";
+    else if (q.dn_dpert && (q.npert < 1 || !(q.eps_pert || q.pert_table))) why = "dn_dpert needs npert >= 1 and eps_pert or pert_table";
+    if (why) {
+      h->err = why;
+      res[i].status = B200MS_ERR_ARG;
+      return B200MS_ERR_ARG;
+    }
+  }
   for (int i = 0; i < nprob && rext2; ++i) {
     if (rext2[i].d2n_dfreq2_deps && !(res[i].d2n_dfreq_deps && rext && rext[i].d4n_dfreq4)) {  // formed from both passes' corrections
       h->err = "d2n_dfreq2_deps needs d2n_dfreq_deps and d4n_dfreq4 of the same problem";
@@ -1863,20 +2091,27 @@ extern "C" int b200ms_solve_batch_ext2(b200ms_handle *h, int nprob, const b200ms
   h->pext = pext;
   h->rext = rext;
   h->rext2 = rext2;
+  h->pert = pert;
   const int rc = solve_batch_impl(h, nprob, prob, res);
   h->pext = nullptr;
   h->rext = nullptr;
   h->rext2 = nullptr;
+  h->pert = nullptr;
   return rc;
+}
+
+extern "C" int b200ms_solve_batch_ext2(b200ms_handle *h, int nprob, const b200ms_problem *prob, b200ms_result *res,
+                                       const b200ms_problem_ext *pext, const b200ms_result_ext *rext, const b200ms_result_ext2 *rext2) {
+  return b200ms_solve_batch_ext3(h, nprob, prob, res, pext, rext, rext2, nullptr);
 }
 
 extern "C" int b200ms_solve_batch_ext(b200ms_handle *h, int nprob, const b200ms_problem *prob, b200ms_result *res,
                                       const b200ms_problem_ext *pext, const b200ms_result_ext *rext) {
-  return b200ms_solve_batch_ext2(h, nprob, prob, res, pext, rext, nullptr);
+  return b200ms_solve_batch_ext3(h, nprob, prob, res, pext, rext, nullptr, nullptr);
 }
 
 extern "C" int b200ms_solve_batch(b200ms_handle *h, int nprob, const b200ms_problem *prob, b200ms_result *res) {
-  return b200ms_solve_batch_ext2(h, nprob, prob, res, nullptr, nullptr, nullptr);
+  return b200ms_solve_batch_ext3(h, nprob, prob, res, nullptr, nullptr, nullptr, nullptr);
 }
 
 // ---- benchmark hook -----------------------------------------------------------------------------------

@@ -146,6 +146,91 @@ __global__ void deriv_final_kernel(const cplx *partial, int nchunk, int count, c
   out[t] = s;
 }
 
+// ------------------------------------------------------------------------------------------------
+// Perturbation responses (b200ms_pert): the permittivity gradients contracted against caller-given fields delta eps_k without
+// writing the maps.  The perturbations of a device batch sit at eps + k kstride + b bstride ([ncomp][N] each; bstride 0 when
+// every problem passes the same field).  The first-order scans sum (per-site gradient) . delta eps_k over a grid-stride chunk
+// for kPertGroup perturbations at a time; the per-site kernels of the group and dispersion passes evaluate their forms once per
+// site and reduce each form . delta eps_k over the block (pert_site_sums).  Every sum of one perturbation is formed in the
+// same order whichever other perturbations share its launch or its device group, and deriv_final_kernel adds the chunks or
+// blocks in a fixed order.
+// ------------------------------------------------------------------------------------------------
+struct PertArgs {
+  const cplx *eps;        // delta eps of perturbation k of problem b at eps + k kstride + b bstride, [ncomp][N]
+  size_t kstride, bstride;
+  int npert;              // perturbations of this launch
+  cplx *partial;          // scans: [B*M][kPertGroup / 3][nchunk][3]; per-site kernels: [B][rows][nblock][3]
+};
+constexpr int kPertGroup = 6;  // perturbations per launch of the first-order scans (accumulators per thread)
+
+// grid (kDerivChunks, B*M), 256 threads: per chunk, sum_g sum_a (w^T dA/d eps_aa(g) v) delta eps_k,a(g) for k < p.npert
+template <typename T, typename C, bool HAS_MU>
+__global__ void __launch_bounds__(256) deriv_pert_kernel(DerivArgs<T, C> a, PertArgs p) {
+  const int M = a.num_modes, bm = blockIdx.y, b = bm / M, m = bm % M;
+  const int ny = a.ny;
+  const size_t N = (size_t)a.nx * ny;
+  const DerivCell<T, C, HAS_MU> c0 = deriv_cell<T, C, HAS_MU>(a, b, m, (const T *)nullptr, (const T *)nullptr, 0.0);
+  const cplx *pe = p.eps + p.bstride * b;
+  cplx s[kPertGroup];
+#pragma unroll
+  for (int k = 0; k < kPertGroup; ++k) s[k] = mk(0.0, 0.0);
+  for (size_t g = (size_t)blockIdx.x * 256 + threadIdx.x; g < N; g += (size_t)gridDim.x * 256) {
+    const int i = (int)(g / ny), j = (int)(g % ny);
+    cplx w1, w2, d[3];
+    c0.w(i, j, w1, w2);
+    c0.eps_grad(i, j, w1, w2, d);
+#pragma unroll
+    for (int k = 0; k < kPertGroup; ++k)
+      if (k < p.npert) {
+        const cplx *e = pe + k * p.kstride + g;
+        s[k] += d[0] * ldg(e) + d[1] * ldg(e + N) + d[2] * ldg(e + 2 * N);
+      }
+  }
+  __shared__ cplx red[kPertGroup][256];
+  for (int k = 0; k < kPertGroup; ++k) red[k][threadIdx.x] = s[k];
+  __syncthreads();
+  for (int h = 128; h > 0; h >>= 1) {
+    if ((int)threadIdx.x < h)
+      for (int k = 0; k < kPertGroup; ++k) red[k][threadIdx.x] += red[k][threadIdx.x + h];
+    __syncthreads();
+  }
+  if (threadIdx.x < kPertGroup)
+    p.partial[(((size_t)bm * (kPertGroup / 3) + threadIdx.x / 3) * gridDim.x + blockIdx.x) * 3 + threadIdx.x % 3] = red[threadIdx.x][0];
+}
+
+// Block sums of the NF per-site forms f[v][a] (a: xx, yy, zz) of site g of problem b against every perturbation of p:
+// value v + NF k of problem b, sum over the block of sum_a f[v][a] delta eps_k,a(g), goes to
+// p.partial[((b rows + (v + NF k) / 3) nblock + block) 3 + (v + NF k) % 3] with rows = ceil(NF npert / 3) (the padding: 0).
+// Every thread of the block calls it; `live` is false for threads outside the grid.
+template <int NF>
+__device__ __forceinline__ void pert_site_sums(const PertArgs &p, int b, size_t g, size_t N, bool live, const cplx (&f)[NF][3]) {
+  __shared__ cplx red[256];
+  const int t = threadIdx.y * blockDim.x + threadIdx.x, nblk = gridDim.x * gridDim.y, blk = blockIdx.y * gridDim.x + blockIdx.x;
+  const int rows = (NF * p.npert + 2) / 3;
+  const cplx *e = p.eps + p.bstride * b + g;
+#pragma unroll 1
+  for (int k = 0; k < p.npert; ++k) {
+#pragma unroll
+    for (int v = 0; v < NF; ++v) {
+      cplx s = mk(0.0, 0.0);
+      if (live) {
+        const cplx *ek = e + k * p.kstride;
+        s = f[v][0] * ldg(ek) + f[v][1] * ldg(ek + N) + f[v][2] * ldg(ek + 2 * N);
+      }
+      red[t] = s;
+      __syncthreads();
+      for (int h = 128; h > 0; h >>= 1) {
+        if (t < h) red[t] += red[t + h];
+        __syncthreads();
+      }
+      const int o = NF * k + v;
+      if (t == 0) p.partial[(((size_t)b * rows + o / 3) * nblk + blk) * 3 + o % 3] = red[0];
+      __syncthreads();
+    }
+  }
+  for (int o = NF * p.npert + t; o < 3 * rows; o += 256) p.partial[(((size_t)b * rows + o / 3) * nblk + blk) * 3 + o % 3] = mk(0.0, 0.0);
+}
+
 // grid like epilogue_kernel: map[b][a][g][m] = (w^T dA/d eps_aa(g) v) * scale[b][m]
 template <typename T, typename C, bool HAS_MU>
 __global__ void __launch_bounds__(256) deriv_map_kernel(DerivArgs<T, C> a) {
@@ -493,9 +578,10 @@ struct GroupCell {
 };
 
 // grid (nchunk, B) x 256 threads (mode 0) or like deriv_map_kernel for one mode slot (mode 1), see above.  ab: [B][2] (alpha,
-// beta); map: [B][3][N][M].
-template <typename T, typename C, bool HAS_MU>
-__global__ void __launch_bounds__(256) group_grad_kernel(DispArgs<T, C> a, int mode, const cplx *ab, cplx *map) {
+// beta); map: [B][3][N][M].  PERT (mode 1 only): instead of the map, the block sums of (chi E + chi' D, chi D) against the
+// perturbations of p (pert_site_sums, NF = 2); the host applies alpha and beta.
+template <typename T, typename C, bool HAS_MU, bool PERT = false>
+__global__ void __launch_bounds__(256) group_grad_kernel(DispArgs<T, C> a, int mode, const cplx *ab, cplx *map, PertArgs p = PertArgs{}) {
   const DerivArgs<T, C> &d = a.d;
   const int nx = d.nx, ny = d.ny, M = d.num_modes;
   const size_t N = (size_t)nx * ny;
@@ -522,8 +608,10 @@ __global__ void __launch_bounds__(256) group_grad_kernel(DispArgs<T, C> a, int m
     if (threadIdx.x < 3) a.partial[((size_t)b * gridDim.x + blockIdx.x) * 3 + threadIdx.x] = threadIdx.x == 0 ? red[0] : mk(0.0, 0.0);
     return;
   }
-  const int j = blockIdx.x * 64 + threadIdx.x, i = blockIdx.y * 4 + threadIdx.y;
-  if (i >= nx || j >= ny) return;
+  const int j0 = blockIdx.x * 64 + threadIdx.x, i0 = blockIdx.y * 4 + threadIdx.y;
+  const bool live = i0 < nx && j0 < ny;
+  if (!PERT && !live) return;
+  const int i = PERT ? min(i0, nx - 1) : i0, j = PERT ? min(j0, ny - 1) : j0;  // PERT: every thread joins the block sums
   const int di[7] = {0, -1, 0, 1, 1, 0, -1}, dj[7] = {0, 0, -1, 0, -1, 1, 1};
   // D_a(w_hat, v) streams over the stencil (only z and w_hat(i, j) are kept); then the w stencil is kept for the other forms
   cplx W[7][2], un[2], hz[3] = {mk(0.0, 0.0), mk(0.0, 0.0), mk(0.0, 0.0)}, h0[2];
@@ -552,15 +640,26 @@ __global__ void __launch_bounds__(256) group_grad_kernel(DispArgs<T, C> a, int m
   const double je = d.jz_e ? d.jz_e[(size_t)b * d.jz_len + (d.jz_axis == 0 ? i : j)] : 1.0;
   const cplx chi[3] = {mk(1.0 / je, 0.0), mk(1.0 / je, 0.0), -(iz * iz) * je};
   const cplx chi1 = a.p1 ? -2.0 * je * (iz * ldg(a.p1 + (size_t)b * 3 * N + 2 * N + g)) : mk(0.0, 0.0);
-  const cplx al = ab[2 * b], be = ab[2 * b + 1];
   const double pec = 0.9 * 1e8;  // PEC-valued input, as eps_grad
   const bool is_pec[3] = {abs2(to_cplx(ldg(G.fb + g))) >= pec * pec, abs2(to_cplx(ldg(G.fb + N + g))) >= pec * pec, abs2(iz) * pec * pec <= 1.0};
-  cplx *o = map + (size_t)b * 3 * N * M;
-  for (int k = 0; k < 3; ++k) {
-    cplx num = chi[k] * e[k], g0 = chi[k] * d0[k];
-    if (k == 2) num += chi1 * d0[k];
-    if (is_pec[k]) num = g0 = mk(0.0, 0.0);
-    o[((size_t)k * N + g) * M + a.q] = al * num + be * g0;
+  if constexpr (PERT) {
+    cplx f[2][3];
+    for (int k = 0; k < 3; ++k) {
+      f[0][k] = chi[k] * e[k];
+      f[1][k] = chi[k] * d0[k];
+      if (k == 2) f[0][k] += chi1 * d0[k];
+      if (is_pec[k]) f[0][k] = f[1][k] = mk(0.0, 0.0);
+    }
+    pert_site_sums<2>(p, b, g, N, live, f);
+  } else {
+    const cplx al = ab[2 * b], be = ab[2 * b + 1];
+    cplx *o = map + (size_t)b * 3 * N * M;
+    for (int k = 0; k < 3; ++k) {
+      cplx num = chi[k] * e[k], g0 = chi[k] * d0[k];
+      if (k == 2) num += chi1 * d0[k];
+      if (is_pec[k]) num = g0 = mk(0.0, 0.0);
+      o[((size_t)k * N + g) * M + a.q] = al * num + be * g0;
+    }
   }
 }
 
@@ -1011,14 +1110,17 @@ __global__ void __launch_bounds__(256) fourth_scan_kernel(DispArgs<T, C> a, Thir
 // ------------------------------------------------------------------------------------------------
 
 // grid like deriv_map_kernel for one mode slot a.q while a.x holds its first-order correction and u.x2 its second-order one;
-// beta: [B][3]; map: [B][3][N][M]
-template <typename T, typename C, bool HAS_MU>
-__global__ void __launch_bounds__(256) disp_grad_kernel(DispArgs<T, C> a, FourthArgs<T> u, const cplx *beta, cplx *map) {
+// beta: [B][3]; map: [B][3][N][M].  PERT: instead of the map, the block sums of (E_0, E_1, E_2) against the perturbations of p
+// (pert_site_sums, NF = 3); the host applies beta_0..beta_2.
+template <typename T, typename C, bool HAS_MU, bool PERT = false>
+__global__ void __launch_bounds__(256) disp_grad_kernel(DispArgs<T, C> a, FourthArgs<T> u, const cplx *beta, cplx *map, PertArgs p = PertArgs{}) {
   const DerivArgs<T, C> &d = a.d;
   const int nx = d.nx, ny = d.ny, M = d.num_modes, b = blockIdx.z;
   const size_t N = (size_t)nx * ny;
-  const int j = blockIdx.x * 64 + threadIdx.x, i = blockIdx.y * 4 + threadIdx.y;
-  if (i >= nx || j >= ny) return;
+  const int j0 = blockIdx.x * 64 + threadIdx.x, i0 = blockIdx.y * 4 + threadIdx.y;
+  const bool live = i0 < nx && j0 < ny;
+  if (!PERT && !live) return;
+  const int i = PERT ? min(i0, nx - 1) : i0, j = PERT ? min(j0, ny - 1) : j0;  // PERT: every thread joins the block sums
   const bool hp = a.p1 != nullptr;
   const T *vb = d.vec + (size_t)a.q * d.vstride + (size_t)b * 2 * N, *xb = a.x + (size_t)b * 2 * N, *x2b = u.x2 + (size_t)b * 2 * N;
   const size_t o4x = (size_t)b * 4 * nx, o4y = (size_t)b * 4 * ny, o3 = (size_t)b * 3 * N;
@@ -1094,18 +1196,33 @@ __global__ void __launch_bounds__(256) disp_grad_kernel(DispArgs<T, C> a, Fourth
   const cplx chi[3] = {mk(1.0 / je, 0.0), mk(1.0 / je, 0.0), -(iz * iz) * je};
   const cplx iz1 = hp ? ldg(a.p1 + o3 + 2 * N + g) : mk(0.0, 0.0), iz2 = hp ? 0.5 * ldg(a.p2 + o3 + 2 * N + g) : mk(0.0, 0.0);
   const cplx chi1 = -2.0 * je * (iz * iz1), chi2 = -je * (2.0 * (iz * iz2) + iz1 * iz1);
-  const cplx be0 = beta[3 * b], be1 = beta[3 * b + 1], be2 = beta[3 * b + 2];
   const double pec = 0.9 * 1e8;  // PEC-valued input, as eps_grad
   const bool is_pec[3] = {abs2(to_cplx(ldg(G.fb + g))) >= pec * pec, abs2(to_cplx(ldg(G.fb + N + g))) >= pec * pec, abs2(iz) * pec * pec <= 1.0};
-  cplx *o = map + (size_t)b * 3 * N * M;
-  for (int k = 0; k < 3; ++k) {
-    cplx e0 = chi[k] * d0[k], e1 = chi[k] * b1[k], e2 = chi[k] * b2[k];
-    if (k == 2) {
-      e1 += chi1 * d0[k];
-      e2 += chi1 * b1[k] + chi2 * d0[k];
+  if constexpr (PERT) {
+    cplx f[3][3];
+    for (int k = 0; k < 3; ++k) {
+      f[0][k] = chi[k] * d0[k];
+      f[1][k] = chi[k] * b1[k];
+      f[2][k] = chi[k] * b2[k];
+      if (k == 2) {
+        f[1][k] += chi1 * d0[k];
+        f[2][k] += chi1 * b1[k] + chi2 * d0[k];
+      }
+      if (is_pec[k]) f[0][k] = f[1][k] = f[2][k] = mk(0.0, 0.0);
     }
-    if (is_pec[k]) e0 = e1 = e2 = mk(0.0, 0.0);
-    o[((size_t)k * N + g) * M + a.q] = be0 * e0 + be1 * e1 + be2 * e2;
+    pert_site_sums<3>(p, b, g, N, live, f);
+  } else {
+    const cplx be0 = beta[3 * b], be1 = beta[3 * b + 1], be2 = beta[3 * b + 2];
+    cplx *o = map + (size_t)b * 3 * N * M;
+    for (int k = 0; k < 3; ++k) {
+      cplx e0 = chi[k] * d0[k], e1 = chi[k] * b1[k], e2 = chi[k] * b2[k];
+      if (k == 2) {
+        e1 += chi1 * d0[k];
+        e2 += chi1 * b1[k] + chi2 * d0[k];
+      }
+      if (is_pec[k]) e0 = e1 = e2 = mk(0.0, 0.0);
+      o[((size_t)k * N + g) * M + a.q] = be0 * e0 + be1 * e1 + be2 * e2;
+    }
   }
 }
 
@@ -1228,6 +1345,43 @@ __global__ void __launch_bounds__(256) tensor_deriv_scan_kernel(TensorDerivArgs<
     __syncthreads();
   }
   if (threadIdx.x < 3) a.partial[((size_t)bm * gridDim.x + blockIdx.x) * 3 + threadIdx.x] = red[threadIdx.x][0];
+}
+
+// grid (nchunk, B*M), 256 threads: per chunk, sum_g sum_c (w^T d mat / d eps_cross[c](g) u) delta eps_k,c(g) for k < p.npert
+// (p: nine components per perturbation), partials laid out as deriv_pert_kernel's
+template <typename C>
+__global__ void __launch_bounds__(256) tensor_pert_kernel(TensorDerivArgs<C> a, PertArgs p) {
+  const int M = a.num_modes, bm = blockIdx.y, b = bm / M, m = bm % M;
+  const int ny = a.ny;
+  const size_t N = (size_t)a.nx * ny;
+  const TensorCell<C> tu = tensor_deriv_cell(a, a.u, b, m, a.cx, a.cy), tw = tensor_deriv_cell(a, a.w, b, m, a.cx, a.cy);
+  const cplx *pe = p.eps + p.bstride * b;
+  cplx s[kPertGroup];
+#pragma unroll
+  for (int k = 0; k < kPertGroup; ++k) s[k] = mk(0.0, 0.0);
+  for (size_t g = (size_t)blockIdx.x * 256 + threadIdx.x; g < N; g += (size_t)gridDim.x * 256) {
+    const int i = (int)(g / ny), j = (int)(g % ny);
+    cplx gr[9];
+    tensor_eps_grad(a, tu, tw, b, i, j, gr);
+#pragma unroll
+    for (int k = 0; k < kPertGroup; ++k)
+      if (k < p.npert) {
+        const cplx *e = pe + k * p.kstride + g;
+        cplx acc = mk(0.0, 0.0);
+        for (int c = 0; c < 9; ++c) acc += gr[c] * ldg(e + (size_t)c * N);
+        s[k] += acc;
+      }
+  }
+  __shared__ cplx red[kPertGroup][256];
+  for (int k = 0; k < kPertGroup; ++k) red[k][threadIdx.x] = s[k];
+  __syncthreads();
+  for (int h = 128; h > 0; h >>= 1) {
+    if ((int)threadIdx.x < h)
+      for (int k = 0; k < kPertGroup; ++k) red[k][threadIdx.x] += red[k][threadIdx.x + h];
+    __syncthreads();
+  }
+  if (threadIdx.x < kPertGroup)
+    p.partial[(((size_t)bm * (kPertGroup / 3) + threadIdx.x / 3) * gridDim.x + blockIdx.x) * 3 + threadIdx.x % 3] = red[threadIdx.x][0];
 }
 
 // grid like epilogue_kernel: map[b][k][g][m] = (w^T d mat / d eps_cross[k](g) u) * scale[b][m]

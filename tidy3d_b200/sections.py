@@ -63,11 +63,13 @@ SHAPE_RECT, SHAPE_DISC, SHAPE_POLYGON = 0, 1, 2
 EpsLike = Union[complex, Sequence[complex], np.ndarray]
 
 
-@dataclass
+@dataclass(eq=False)
 class Medium:
     """Relative permittivity of a medium: a scalar (isotropic), three numbers (diagonal, ``AnisotropicMedium``), a 3x3
     tensor (``FullyAnisotropicMedium``), or a callable ``freq -> any of those`` for dispersive media (the reference
-    evaluates ``structure.eps_comp(row, col, frequency)``, simulation.py:1176-1185)."""
+    evaluates ``structure.eps_comp(row, col, frequency)``, simulation.py:1176-1185).  A medium is identified by the object, as
+    ``Section`` does, so that it can key the per-medium dicts of ``eps_pert``: ``==`` and ``hash`` are those of the object, and
+    two media with equal ``eps`` compare unequal (up to version 211 without ``eps_pert``, ``==`` compared ``eps``)."""
 
     eps: Union[EpsLike, Callable[[float], EpsLike]]
 
@@ -189,6 +191,23 @@ class Section:
         if not any(callable(m.eps) for m in media):
             return None
         return np.ascontiguousarray([m.d4tensor_dfreq4(freq).ravel() for m in media], dtype=np.complex128)
+
+    def pert_table(self, perts) -> np.ndarray:
+        """(K, nmedia, 9) complex128 perturbation table of ``eps_pert`` (a sequence of K dicts ``{Medium: change of its eps}``, a
+        scalar, three numbers or a 3x3 tensor; media not named change by 0) in the medium order of ``pack``'s ``eps_table``."""
+        media, _ = self._media()
+        if isinstance(perts, dict) or not isinstance(perts, (list, tuple)) or not perts or not all(isinstance(d, dict) for d in perts):
+            raise ValueError("a section's eps_pert is a non-empty sequence of dicts {Medium: change of its eps}")
+        table = np.zeros((len(perts), len(media), 9), dtype=np.complex128)
+        for k, d in enumerate(perts):
+            for m, v in d.items():
+                idx = next((i for i, known in enumerate(media) if known is m), None)
+                if idx is None:
+                    raise ValueError("eps_pert names a medium that is not part of the section")
+                if callable(v):
+                    raise ValueError("eps_pert gives the change of eps at the solve's frequency: a number or a tensor, not a callable")
+                table[k, idx] = Medium(v).tensor(0.0).ravel()
+        return table
 
     def pack(self, freq: float, shape: Optional[Tuple[int, int]] = None, dispersion: bool = False, second: bool = False,
              third: bool = False):

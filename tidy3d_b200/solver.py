@@ -137,15 +137,42 @@ def compute_modes_batch(
     left eigenvector could not be paired with it gets NaN; ``left_paired`` in the info dict counts the modes that were (num_modes
     for diagonal problems, -1 without derivatives).  Diagonal problems solve as without the flag and report ``dn_deps`` as
     (3, Nx, Ny, M).  With it, ``"freq2"``, ``"group_eps"`` and ``"freq3"`` still raise on tensorial problems.
+
+    ``"pert"``, ``"group_pert"`` and ``"disp_pert"`` contract the maps of ``"eps"``, ``"group_eps"`` and ``"disp_eps"`` on the
+    device against K caller-given permittivity perturbations, so that no per-cell map is written or copied: each problem may carry
+    ``eps_pert=``, a complex (K, 9, Nx, Ny) array in the layout of ``eps_cross`` ((9, Nx, Ny): K = 1; diagonal problems read
+    xx, yy, zz, tensorial ones with ``left_solve=True`` all nine), or for a ``section`` a sequence of K dicts
+    ``{Medium: scalar | 3 numbers | (3, 3) tensor}``, the change of each named medium's eps (others: 0), rasterised on the device
+    like its permittivity.  Problems that pass the same array object share one upload.  Each kind takes the solves of the map
+    kind it contracts, not its map, and adds (K, M) arrays to the info dict: ``"pert"`` ``dn_dpert``, d(n_eff + i k_eff) per unit
+    amplitude of delta eps_k; ``"group_pert"`` (implies ``"pert"`` and ``"freq2"``) ``d2n_dfreq_dpert`` (1/Hz) and ``dng_dpert`` =
+    Re ``dn_dpert`` + f Re ``d2n_dfreq_dpert``, the response of ``n_group`` (also for a complex delta eps); ``"disp_pert"``
+    (implies ``"group_pert"`` and ``"freq4"``) ``d2n_dfreq2_dpert`` (1/Hz^2) and ``dispersion_dpert`` (ps/(nm km) per unit
+    amplitude, ``plugin.dispersion_gradient_of``).  Every response is taken at fixed PML stretch, mu, d eps / df and
+    d^2 eps / df^2: a perturbation of the material dispersion itself is not modelled.  Scope and NaNs follow the contracted map:
+    ``"group_pert"`` and ``"disp_pert"`` raise on tensorial problems, ``"pert"`` needs ``left_solve=True`` there.  Problems without
+    ``eps_pert`` get none of these keys; maps and contractions may be asked for together.
     """
     post = tuple(post or ())
     unknown = set(post) - {"gauge", "normalize", "flux", "overlaps"}
     if unknown:
         raise ValueError(f"unknown post-processing step(s): {sorted(unknown)}")
     derivatives = tuple(derivatives or ())
-    unknown = set(derivatives) - {"freq", "eps", "freq2", "group_eps", "freq3", "freq4", "disp_eps"}
+    unknown = set(derivatives) - {"freq", "eps", "freq2", "group_eps", "freq3", "freq4", "disp_eps", "pert", "group_pert", "disp_pert"}
     if unknown:
         raise ValueError(f"unknown derivative(s): {sorted(unknown)}")
+    has_pert = [p.get("eps_pert") is not None for p in problems]
+    if any(has_pert) and not {"pert", "group_pert", "disp_pert"} & set(derivatives):
+        raise ValueError("eps_pert is read by derivatives=(\"pert\",), (\"group_pert\",) or (\"disp_pert\",): ask for one of them")
+    if {"pert", "group_pert", "disp_pert"} & set(derivatives) and not any(has_pert):
+        raise ValueError("derivatives \"pert\", \"group_pert\" and \"disp_pert\" contract against eps_pert: no problem gives it")
+    disp_pert = "disp_pert" in derivatives
+    if disp_pert:
+        derivatives = derivatives + tuple(d for d in ("group_pert", "freq4") if d not in derivatives)
+    group_pert = "group_pert" in derivatives
+    if group_pert:
+        derivatives = derivatives + tuple(d for d in ("pert", "freq2") if d not in derivatives)
+    want_pert = "pert" in derivatives
     if left_solve and not derivatives:
         raise ValueError("left_solve=True serves derivatives=(\"freq\", \"eps\") of tensorial problems: ask for derivatives as well")
     disp_eps = "disp_eps" in derivatives
@@ -164,7 +191,7 @@ def compute_modes_batch(
     if second and "freq" not in derivatives:
         derivatives = derivatives + ("freq",)
     post_flags = (1 if "gauge" in post else 0) | (2 if "normalize" in post else 0)
-    packed, cache = [], {}
+    packed, cache, pcache = [], {}, {}
     for p in problems:
         split = p.get("split_curl_scaling")
         target_override = None
@@ -189,7 +216,10 @@ def compute_modes_batch(
             post=post_flags, grid_correction=p.get("grid_correction"), plane_bounds=p.get("plane_bounds"),
             eps_dfreq=p.get("eps_dfreq"), derivatives="freq" in derivatives, eps_d2freq=p.get("eps_d2freq"), second=second,
             eps_d3freq=p.get("eps_d3freq"), third=third, left_solve=left_solve, eps_d4freq=p.get("eps_d4freq"), fourth=fourth,
+            eps_pert=p.get("eps_pert"), eps_pert_packed=None if section is not None else pcache.get(id(p.get("eps_pert"))),
         )  # fmt: skip
+        if pk.eps_pert is not None:  # problems that pass the same eps_pert object share one array (one device copy)
+            pcache[id(p["eps_pert"])] = pk.eps_pert
         if split is None and section is None:
             cache[key] = pk.eps
         if section is None and key in cache and len(packed) and packed[-1].eps is pk.eps:
@@ -204,7 +234,7 @@ def compute_modes_batch(
         want_eps = "eps" in derivatives
         dkw = dict(want_dfreq="freq" in derivatives, want_deps=want_eps and not left_solve, want_deps_tensor=want_eps and left_solve,
                    want_d2freq=second, want_group_eps=group_eps, want_d3freq=third, want_d4freq=fourth,
-                   want_d2freq2_deps=disp_eps) if derivatives else {}
+                   want_d2freq2_deps=disp_eps, want_pert=want_pert, want_group_pert=group_pert, want_disp_pert=disp_pert) if derivatives else {}
         rc, fields, ncs, results = h.solve_batch(packed, want_fields, fields_ptrs, want_flux=("flux" in post or "normalize" in post),
                                                  want_overlaps="overlaps" in post, **dkw)
         flux_out, te_out, ov_out = h.last_flux, h.last_te, h.last_overlaps
@@ -214,6 +244,7 @@ def compute_modes_batch(
         d3_out = h.last_d3n_dfreq3 if third else []
         d4_out, d4res_out = (h.last_d4n_dfreq4, h.last_d4n_residual) if fourth else ([], [])
         dmap_out = h.last_d2n_dfreq2_deps if disp_eps else []
+        pert_out = (h.last_dn_dpert, h.last_d2n_dfreq_dpert, h.last_d2n_dfreq2_dpert) if want_pert else ([], [], [])
         err = h.last_error() if rc != _cabi.OK else ""
     if rc != _cabi.OK:
         bad = [i for i in range(len(packed)) if results[i].status != _cabi.OK]
@@ -268,6 +299,17 @@ def compute_modes_batch(
 
             infos[-1]["d2n_dfreq2_deps"] = dmap_out[i]
             infos[-1]["dispersion_deps"] = dispersion_gradient_of(float(packed[i].struct.freq), gmap_out[i], dmap_out[i])
+        if pert_out[0] and pert_out[0][i] is not None:
+            fq = float(packed[i].struct.freq)
+            infos[-1]["dn_dpert"] = pert_out[0][i]
+            if group_pert:
+                infos[-1]["d2n_dfreq_dpert"] = pert_out[1][i]
+                infos[-1]["dng_dpert"] = pert_out[0][i].real + fq * pert_out[1][i].real
+            if disp_pert:
+                from .plugin import dispersion_gradient_of  # noqa: PLC0415  (plugin imports this module)
+
+                infos[-1]["d2n_dfreq2_dpert"] = pert_out[2][i]
+                infos[-1]["dispersion_dpert"] = dispersion_gradient_of(fq, pert_out[1][i], pert_out[2][i])
     return (out, infos) if return_info else out
 
 
