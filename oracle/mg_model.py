@@ -30,7 +30,7 @@ class Opts:
     """The b200ms_options fields the multigrid depends on (defaults of b200ms_default_options)."""
 
     FIELDS = dict(mg_min_size=12, mg_nu=2, mg_omega=0.8, mg_coarse_iters=16, mg_ppw=4.0, mg_pml_phase=np.pi / 4, mg_precision=1,
-                  ncv=0, gmres_restart=40, inner_mode=1)
+                  ncv=0, gmres_restart=40)
 
     def __init__(self, src=None, **kw):
         for k, v in self.FIELDS.items():
@@ -358,9 +358,7 @@ class Multigrid:
         m = min(ncv, length - 1)
         if m < prob.num_modes + 2:
             m = min(prob.num_modes + 2, length)
-        restart = max(2, o.gmres_restart)
-        if o.inner_mode != 0:
-            restart = min(restart, GS_MAX_COEF - 4)
+        restart = min(max(2, o.gmres_restart), GS_MAX_COEF - 4)
         self.kc = max(2, min(o.mg_coarse_iters, max(m, restart) - 1))
 
     @property

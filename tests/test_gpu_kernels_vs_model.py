@@ -249,7 +249,7 @@ def check_solve(h, pks, probs, wls, kws, rng):
         _observe("solve true/tol", true / tol)
         assert true <= 1.25 * tol, (q, true, est[q])
         o = h.options
-        if o.inner_mode == 0 or o.mg_precision == 0 or o.inner_ir == 0 or probs[q].masked or probs[q].tensorial:
+        if o.mg_precision == 0 or o.inner_ir == 0 or probs[q].masked or probs[q].tensorial:
             # fp64 cycles only (BatchSolver::solve_op, fgmres): the reported residual is the Givens estimate or the fp64
             # residual, both the true residual up to rounding
             _observe("solve fp64 |true - est| / true", abs(true - est[q]) / true)
@@ -262,7 +262,7 @@ def check_solve(h, pks, probs, wls, kws, rng):
 
 @pytest.mark.parametrize("name", SOLVE_CASES)
 @pytest.mark.parametrize("ir", [1, 0])
-def test_inner_solve_reaches_inner_tol(handles, name, ir):
+def test_inner_solve_reaches_and_reports_inner_tol(handles, name, ir):
     wl, kw = mg_cases.case(name)
     check_solve(handles["fp32" if ir else "ir0"], [mg_cases.packed(_cabi, wl, kw)], [mg_cases.model_problem(wl, kw)], [wl], [kw],
                 np.random.default_rng(4))
@@ -294,7 +294,7 @@ BATCHES = {
 
 
 @pytest.mark.parametrize("bname", list(BATCHES))
-def test_batched_kernels_match_model_and_single_problem(handles, bname):
+def test_production_batches_match_model_and_single_problem(handles, bname):
     pks, probs, wls, kws = BATCHES[bname]()
     real = mg_cases.is_real(wls[0], kws[0])
     nb = len(pks)

@@ -147,8 +147,8 @@ def test_pec_cells_report_zero():
     assert (out["d2n_dfreq2_deps"][:, 0, 5] == 0).all() and np.abs(out["d2n_dfreq2_deps"]).max() > 0
 
 
-def test_ext2_struct_mirrors_the_header():
-    assert _cabi.ABI_VERSION == 211
+def test_ext2_struct_mirrors_the_v212_header():
+    assert _cabi.ABI_VERSION == 212
     assert [f for f, _ in _cabi.ResultExt2._fields_] == _header_fields("b200ms_result_ext2") == ["d2n_dfreq2_deps"]
     assert [f for f, _ in _cabi.ResultExt._fields_] == _header_fields("b200ms_result_ext") == ["d4n_dfreq4", "d4n_residual"]
     assert "b200ms_solve_batch_ext2" in _cabi.EXPORTS

@@ -64,11 +64,6 @@ struct b200ms_handle {
   DevBuf deriv;       // tables, partial sums, dispersion input and d n / d eps map of the derivative pass
   DevBuf disp;        // tables, material directions and partial sums of the dispersion pass
   DevBuf pert_dev;    // perturbation fields of a device batch and the partial sums of their contraction (b200ms_pert)
-  DevBuf warm;        // sorted Ritz vectors of the previous device batch of this call ([k][B][len]): warm start of the next one
-  int warm_B = 0, warm_k = 0, warm_tsize = 0;
-  size_t warm_len = 0;
-  bool warm_valid = false;
-  long long warm_key[16];
   b200ms_options opt;
   std::string err;
   cudaEvent_t ev0 = nullptr, ev1 = nullptr;
@@ -106,7 +101,6 @@ extern "C" void b200ms_default_options(b200ms_options *o) {
   o->gmres_cgs2 = 2;
   o->inner_relax = 1.0;
   o->inner_relax_cap = 1e-4;
-  o->inner_mode = 1;
   o->inner_ir = 1;
   o->ir_floor = 1e-4;
   o->ir_trust = 3e-5;
@@ -114,13 +108,10 @@ extern "C" void b200ms_default_options(b200ms_options *o) {
   o->cluster_gap = 1e-3;
   o->mg_fuse_first = 1;
   o->ks_keep = 0;
-  o->transfer_tiled = 0;
-  o->warm_start = 0;
   o->mg_fused_tail = 1;
-  o->stencil_async = 0;
   o->kappa_cap = 1e4;
   o->outer_dgks = 1;
-  o->stencil_pair = 4;
+  o->stencil_pair = 1;
   o->stencil_pair_rows = 0;
   o->transfer_vec = 15;
   o->tensor_mg_cycles = 3;
@@ -160,7 +151,6 @@ extern "C" int b200ms_destroy(b200ms_handle *h) {
   h->scan.release();
   h->refs.release();
   h->post.release();
-  h->warm.release();
   h->deriv.release();
   h->disp.release();
   h->pert_dev.release();
@@ -188,6 +178,7 @@ extern "C" void b200ms_host_free(void *ptr) {
 
 extern "C" int b200ms_set_options(b200ms_handle *h, const b200ms_options *opt) {
   if (!h || !opt) return B200MS_ERR_ARG;
+  if (opt->stencil_variant < 0 || opt->stencil_variant > 1 || opt->stencil_pair < 0 || opt->stencil_pair > 1) return B200MS_ERR_ARG;
   h->opt = *opt;
   return B200MS_OK;
 }
@@ -1226,9 +1217,9 @@ void tensor_derivative_pass(b200ms_handle *h, BatchSolver<T, C, P, PC> &S, const
 // writes r2 from the same x, a second correction solve (A - lambda_q) x2 = r2 runs at the same shift, and fourth_scan_kernel
 // sums the products of lambda''''.  With b200ms_result_ext2.d2n_dfreq2_deps (which needs d2n_dfreq_deps and d4n_dfreq4),
 // disp_grad_kernel then writes slot q of the map d_g (d^2n/df^2) from the same x and x2.  It writes its own buffers, the
-// first four slots of the outer Krylov basis and the inner solver's scratch -- nothing the fields, the post-processing or the
-// warm start read.  b200ms_pert.d2n_dfreq_dpert / d2n_dfreq2_dpert run the PERT instantiations of the same two kernels at the
-// same points (pert_second_order), in place of or beside the maps.
+// first four slots of the outer Krylov basis and the inner solver's scratch -- nothing the fields or the post-processing read.
+// b200ms_pert.d2n_dfreq_dpert / d2n_dfreq2_dpert run the PERT instantiations of the same two kernels at the same points
+// (pert_second_order), in place of or beside the maps.
 template <typename T, typename C, typename P, typename PC>
 void dispersion_pass(b200ms_handle *h, BatchSolver<T, C, P, PC> &S, const std::vector<const ProblemSetup *> &ps, const std::vector<int> &ids,
                      const Window &W, const b200ms_problem *prob, b200ms_result *res, const std::vector<cd> &nsorted,
@@ -1722,14 +1713,7 @@ void solve_group(b200ms_handle *h, const std::vector<int> &ids, const Window &W,
     eig.nconv.assign(B, k);
     eig.resid.assign(B, 0.0);
   } else {
-    // consecutive device batches of one call are neighbouring slices of a sweep: start each problem's Krylov space from the
-    // wanted Ritz vectors of the problem at the same position of the previous batch (same group key, same shapes)
-    long long key[16] = {S.nx, S.ny, k, (long long)sizeof(T), S.tensor_ ? 1 : 0, S.has_mu ? 1 : 0, ps[0]->ax[0].pmc, ps[0]->ax[1].pmc,
-                         ps[0]->direction, ps[0]->masked ? 1 : 0, (long long)S.len, 0, 0, 0, 0, 0};
-    const bool warm = h->opt.warm_start && h->warm_valid && h->warm_B >= B && h->warm_k == k && h->warm_len == S.len &&
-                      h->warm_tsize == (int)sizeof(T) && std::memcmp(key, h->warm_key, sizeof(key)) == 0;
-    if (warm) S.init_start_from(reinterpret_cast<const T *>(h->warm.p), h->warm_B);
-    else S.init_start_vector(0);
+    S.init_start_vector(0);
     NvtxRange r("b200ms:eigen-iteration");
     eig = S.krylov_schur(real_arith);
   }
@@ -1777,16 +1761,6 @@ void solve_group(b200ms_handle *h, const std::vector<int> &ids, const Window &W,
       auto r = S.eigen_residuals(q, lq);
       for (int b = 0; b < B; ++b) maxres[b] = std::max(maxres[b], r[b]);
     }
-  }
-  if (h->opt.warm_start && !relative) {  // keep the sorted Ritz vectors for the next batch of this call
-    long long key[16] = {S.nx, S.ny, k, (long long)sizeof(T), S.tensor_ ? 1 : 0, S.has_mu ? 1 : 0, ps[0]->ax[0].pmc, ps[0]->ax[1].pmc,
-                         ps[0]->direction, ps[0]->masked ? 1 : 0, (long long)S.len, 0, 0, 0, 0, 0};
-    const size_t bytes = (size_t)k * S.vstride * sizeof(T);
-    h->warm.reserve(bytes + 256);
-    CUDA_CHECK(cudaMemcpyAsync(h->warm.p, S.ritz_ptr(), bytes, cudaMemcpyDeviceToDevice, h->stream));
-    std::memcpy(h->warm_key, key, sizeof(key));
-    h->warm_B = B; h->warm_k = k; h->warm_len = S.len; h->warm_tsize = (int)sizeof(T);
-    h->warm_valid = true;
   }
   // the forward solve's counters, before any derivative pass runs more solves in this batch
   const SolveStats fwd = S.stats;
@@ -1895,7 +1869,6 @@ static int solve_batch_impl(b200ms_handle *h, int nprob, const b200ms_problem *p
   h->err.clear();
   std::memset(&h->stats, 0, sizeof(h->stats));
   h->stats.nprob = nprob;
-  h->warm_valid = false;  // warm starts never cross calls: a call's results depend on its own inputs only
   const auto call0 = std::chrono::steady_clock::now();
   int first_err = B200MS_OK;
   try {

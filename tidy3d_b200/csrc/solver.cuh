@@ -168,8 +168,7 @@ class BatchSolver {
     const int ncv = opt_.ncv > 0 ? opt_.ncv : std::max(2 * k + 1, 20);
     m = std::min(ncv, (int)std::min<size_t>(len - 1, 1 << 20));
     if (m < k + 2) m = std::min<int>(k + 2, (int)len);
-    restart = std::max(2, opt_.gmres_restart);
-    if (opt_.inner_mode != 0) restart = std::min(restart, kGsMaxCoef - 4);
+    restart = std::min(std::max(2, opt_.gmres_restart), kGsMaxCoef - 4);
     mask_x_ = (!p0.ax[0].pmc && nx > 1) ? 1 : 0;
     mask_y_ = (!p0.ax[1].pmc && ny > 1) ? 1 : 0;
     {  // lincomb_kernel stages up to m x m coefficients per CTA: beyond the 48 KB default it has to opt in (see lincomb)
@@ -531,7 +530,7 @@ class BatchSolver {
       // rows marched per CTA: the march is a serial chain of (TXR + 3) row steps, each waiting on one global-load
       // round trip, so small levels (few CTAs per SM, nothing to hide that latency behind) get short chains
       bool rows32 = v.nx >= 384;
-      if (rows32 && opt_.stencil_variant != 2 && opt_.stencil_variant != 3) {
+      if (rows32) {
         // wave quantisation: 7 CTAs of 128 threads per SM are resident; when 32-row CTAs leave the last wave mostly empty
         // (e.g. 32 problems of 512^2: 2.47 waves) 16-row CTAs fill it at the price of 9 % more halo rows
         const double per_wave = sms_ * 7.0;
@@ -540,7 +539,7 @@ class BatchSolver {
         const double t32 = std::ceil(c32) * 35.0, t16 = std::ceil(c16) * 19.0;  // waves x row steps per CTA
         if (t16 < 0.97 * t32) rows32 = false;
       }
-      if (rows32 || opt_.stencil_variant == 2) launch_march<TT, CC, 32>(v, mode, a, dinv != nullptr);
+      if (rows32) launch_march<TT, CC, 32>(v, mode, a, dinv != nullptr);
       else if (v.nx >= 192) launch_march<TT, CC, 16>(v, mode, a, dinv != nullptr);
       else launch_march<TT, CC, 8>(v, mode, a, dinv != nullptr);
       return;
@@ -558,12 +557,12 @@ class BatchSolver {
     }
   }
   // pair-marching kernels (csrc/march2.cuh, csrc/march2_tma.cuh): real fp32 multigrid operators without mu fields on even-width
-  // levels.  stencil_pair: 1 / 2 = register version with one / two rows of prefetch registers; 3 / 4 = TMA row staging (ring of
-  // three stages) where it applies (ny % 4 == 0, not the fused first sweeps), register version 1 / 2 elsewhere; 5 = TMA with two stages.
+  // levels (stencil_pair = 1).  TMA row staging (ring of three stages) where it applies (ny % 4 == 0, not the fused first
+  // sweeps), the register version with two rows of prefetch registers elsewhere.
   using March2Fn = void (*)(StencilArgs<float, float>, int);
   struct March2Pick {
     March2Fn fn = nullptr;
-    int stages = 0, narr = 0, id = 0;  // stages > 0: TMA version with that ring depth
+    int stages = 0, narr = 0;  // stages > 0: TMA version with that ring depth
   };
   // the most recent pair-kernel launch, kept so that the V-cycle graph can redirect the output of its last sweep
   struct M2Launch {
@@ -578,36 +577,18 @@ class BatchSolver {
   M2Launch last_m2_;
   March2Pick march2_pick(int md, int ny) const {
     March2Pick p;
-    const int sp = opt_.stencil_pair;
-    const int pf = (sp == 2 || sp == 4) ? 2 : 1;
-    const int stages = (sp == 3 || sp == 4) ? 3 : (sp == 5 ? 2 : 0);
-    if (stages > 0 && (ny % 4) == 0 && md != MODE_JACOBI_D0) {
-      p.stages = stages;
+    if ((ny % 4) == 0 && md != MODE_JACOBI_D0) {
+      p.stages = 3;
       p.narr = md == MODE_APPLY ? 5 : (md == MODE_RESID ? 7 : 9);
-      p.id = 16 + stages;
-      if (stages == 3) {
-        if (md == MODE_APPLY) p.fn = stencil_march2_tma_kernel<MODE_APPLY, 3>;
-        else if (md == MODE_RESID) p.fn = stencil_march2_tma_kernel<MODE_RESID, 3>;
-        else if (md == MODE_JACOBI_D) p.fn = stencil_march2_tma_kernel<MODE_JACOBI_D, 3>;
-      } else {
-        if (md == MODE_APPLY) p.fn = stencil_march2_tma_kernel<MODE_APPLY, 2>;
-        else if (md == MODE_RESID) p.fn = stencil_march2_tma_kernel<MODE_RESID, 2>;
-        else if (md == MODE_JACOBI_D) p.fn = stencil_march2_tma_kernel<MODE_JACOBI_D, 2>;
-      }
+      if (md == MODE_APPLY) p.fn = stencil_march2_tma_kernel<MODE_APPLY, 3>;
+      else if (md == MODE_RESID) p.fn = stencil_march2_tma_kernel<MODE_RESID, 3>;
+      else if (md == MODE_JACOBI_D) p.fn = stencil_march2_tma_kernel<MODE_JACOBI_D, 3>;
       return p;
     }
-    p.id = pf;
-    if (pf == 1) {
-      if (md == MODE_APPLY) p.fn = stencil_march2_kernel<float, MODE_APPLY, 1>;
-      else if (md == MODE_RESID) p.fn = stencil_march2_kernel<float, MODE_RESID, 1>;
-      else if (md == MODE_JACOBI_D) p.fn = stencil_march2_kernel<float, MODE_JACOBI_D, 1>;
-      else if (md == MODE_JACOBI_D0) p.fn = stencil_march2_kernel<float, MODE_JACOBI_D0, 1>;
-    } else {
-      if (md == MODE_APPLY) p.fn = stencil_march2_kernel<float, MODE_APPLY, 2>;
-      else if (md == MODE_RESID) p.fn = stencil_march2_kernel<float, MODE_RESID, 2>;
-      else if (md == MODE_JACOBI_D) p.fn = stencil_march2_kernel<float, MODE_JACOBI_D, 2>;
-      else if (md == MODE_JACOBI_D0) p.fn = stencil_march2_kernel<float, MODE_JACOBI_D0, 2>;
-    }
+    if (md == MODE_APPLY) p.fn = stencil_march2_kernel<float, MODE_APPLY, 2>;
+    else if (md == MODE_RESID) p.fn = stencil_march2_kernel<float, MODE_RESID, 2>;
+    else if (md == MODE_JACOBI_D) p.fn = stencil_march2_kernel<float, MODE_JACOBI_D, 2>;
+    else if (md == MODE_JACOBI_D0) p.fn = stencil_march2_kernel<float, MODE_JACOBI_D0, 2>;
     return p;
   }
   bool march2_eligible(const Level &v) const {
@@ -616,7 +597,7 @@ class BatchSolver {
   static size_t march2_smem(const March2Pick &p, int W) { return (size_t)p.stages * p.narr * W * sizeof(float2); }
   // resident CTAs on the device for this kernel at this CTA width; also raises the kernel's dynamic shared-memory limit once
   int march2_resident(const March2Pick &p, int md, int W) {
-    const long key = ((long)md * 32 + p.id) * 1024 + W;
+    const long key = ((long)md * 32 + p.stages) * 1024 + W;
     auto it = m2_resident_.find(key);
     if (it == m2_resident_.end()) {
       int per_sm = 0;
@@ -648,10 +629,7 @@ class BatchSolver {
   }
   March2Pick resid_restrict_pick(int ny) const {
     March2Pick p = march2_pick(MODE_RESID, ny);
-    if (p.stages == 3) p.fn = stencil_march2_tma_kernel<MODE_RESID_RESTRICT, 3>;
-    else if (p.stages == 2) p.fn = stencil_march2_tma_kernel<MODE_RESID_RESTRICT, 2>;
-    else p.fn = nullptr;
-    p.id = 32 + p.stages;
+    p.fn = p.stages ? stencil_march2_tma_kernel<MODE_RESID_RESTRICT, 3> : nullptr;
     return p;
   }
   // Coarse rows per CTA of the fused residual + restriction on level l (csrc/march2_tma.cuh), or 0 where it does not apply:
@@ -661,7 +639,7 @@ class BatchSolver {
   int resid_restrict_plan(int l, int W, int nstrips) {
     const Level &v = lv[l];
     const TransferArgs &t = v.tr;
-    if (!(opt_.transfer_vec & 4) || !(opt_.transfer_vec & 2) || opt_.transfer_tiled || nstrips != 1 || v.ny > 2 * kM2MaxW) return 0;
+    if (!(opt_.transfer_vec & 4) || !(opt_.transfer_vec & 2) || nstrips != 1 || v.ny > 2 * kM2MaxW) return 0;
     if (!t.xn.r4 || !t.xe.r4 || !t.yn.r4 || !t.ye.r4) return 0;
     const March2Pick p = resid_restrict_pick(v.ny);
     if (!p.fn) return 0;
@@ -699,7 +677,7 @@ class BatchSolver {
       return worst;
     };
     const size_t smem = march2_smem(p, W) + rr_smem_extra(v.ny);
-    const long key = ((long)MODE_RESID_RESTRICT * 32 + p.id) * 1024 + W;
+    const long key = ((long)MODE_RESID_RESTRICT * 32 + p.stages) * 1024 + W;
     auto it = m2_resident_.find(key);
     if (it == m2_resident_.end()) {
       int per_sm = 0;
@@ -837,15 +815,6 @@ class BatchSolver {
   template <typename TT, typename CC, int TXR>
   void launch_march(const Level &v, int mode, const StencilArgs<TT, CC> &a, bool have_dinv) {
     dim3 blk(kMarchCols), grd((v.ny + kMarchOut - 1) / kMarchOut, (v.nx + TXR - 1) / TXR, B);
-    if constexpr (sizeof(TT) <= 8 && sizeof(CC) <= 8) {
-      // cp.async (LDGSTS) variant: the multigrid hot path -- stored-diagonal sweep, residual, apply -- without mu fields
-      if (opt_.stencil_async && !has_mu && mode != MODE_JACOBI_D0 && (mode != MODE_JACOBI || have_dinv)) {
-        if (mode == MODE_JACOBI) stencil_march_async_kernel<TT, CC, MODE_JACOBI_D, TXR><<<grd, blk, 0, st_>>>(a);
-        else if (mode == MODE_RESID) stencil_march_async_kernel<TT, CC, MODE_RESID, TXR><<<grd, blk, 0, st_>>>(a);
-        else stencil_march_async_kernel<TT, CC, MODE_APPLY, TXR><<<grd, blk, 0, st_>>>(a);
-        return;
-      }
-    }
     if (mode == MODE_JACOBI_D0) {  // two sweeps from zero in one pass (needs the stored diagonal)
       if (has_mu) stencil_march_kernel<TT, CC, MODE_JACOBI_D0, true, TXR><<<grd, blk, 0, st_>>>(a);
       else stencil_march_kernel<TT, CC, MODE_JACOBI_D0, false, TXR><<<grd, blk, 0, st_>>>(a);
@@ -1193,19 +1162,12 @@ class BatchSolver {
     } else {
       apply(l, MODE_RESID, cur, rin, v.r);
       const TransferArgs &t = v.tr;
-      dim3 blk(64, 4);
+      dim3 blk(64, 4), grd((t.nyc + 63) / 64, (t.nxc + 3) / 4, 2 * B);
       if constexpr (sizeof(P) <= 8) {
-        if (opt_.transfer_tiled && t.nyc >= 64) {
-          dim3 grd((t.nyc + kRtJ - 1) / kRtJ, (t.nxc + kRtI - 1) / kRtI, 2 * B);
-          restrict_tiled_kernel<P><<<grd, blk, 0, st_>>>(t, v.r, lv[l + 1].b);
-        } else {
-          dim3 grd((t.nyc + 63) / 64, (t.nxc + 3) / 4, 2 * B);
-          const bool packed = (opt_.transfer_vec & 2) && std::is_same<typename RealOf<P>::type, float>::value && t.xn.r4 && t.xe.r4 && t.yn.r4 && t.ye.r4;
-          if (packed) restrict4_kernel<P><<<grd, blk, 0, st_>>>(t, v.r, lv[l + 1].b);
-          else restrict_kernel<P><<<grd, blk, 0, st_>>>(t, v.r, lv[l + 1].b);
-        }
+        const bool packed = (opt_.transfer_vec & 2) && std::is_same<typename RealOf<P>::type, float>::value && t.xn.r4 && t.xe.r4 && t.yn.r4 && t.ye.r4;
+        if (packed) restrict4_kernel<P><<<grd, blk, 0, st_>>>(t, v.r, lv[l + 1].b);
+        else restrict_kernel<P><<<grd, blk, 0, st_>>>(t, v.r, lv[l + 1].b);
       } else {
-        dim3 grd((t.nyc + 63) / 64, (t.nxc + 3) / 4, 2 * B);
         restrict_kernel<P><<<grd, blk, 0, st_>>>(t, v.r, lv[l + 1].b);
       }
       stats.launches++;
@@ -1230,7 +1192,7 @@ class BatchSolver {
   void prolong_add(int l, P *fine) {
     const TransferArgs &t = lv[l].tr;
     stats.launches++;
-    if (t.nyf >= 256 && opt_.transfer_tiled != 2) {  // four fine columns per thread
+    if (t.nyf >= 256) {  // four fine columns per thread
       dim3 blk(64, 4), grd((t.nyf + 255) / 256, (t.nxf + 3) / 4, 2 * B);
       if ((opt_.transfer_vec & 1) && std::is_same<P, float>::value && (t.nyf % 4) == 0) prolong_add4_kernel<P, true><<<grd, blk, 0, st_>>>(t, lv[l + 1].x, fine);
       else prolong_add4_kernel<P, false><<<grd, blk, 0, st_>>>(t, lv[l + 1].x, fine);
@@ -1722,9 +1684,9 @@ class BatchSolver {
   // res_out: the final relative residual of every problem
   double solve_op(const T *rhs, T *xsol, int &iters_out, const std::vector<char> *skip = nullptr, const std::vector<double> *tolv = nullptr,
                   std::vector<double> *res_out = nullptr) {
-    // the tensorial path stays on the round-1 host-driven fp64 FGMRES: with no fp32 cycles to gain from, its adaptive
-    // one-pass Gram-Schmidt is ~10 % faster than always-CGS2 device cycles (angled_64: 2 109 vs 2 322 ms)
-    if (opt_.inner_mode == 0 || tensor_) return fgmres(rhs, xsol, iters_out, skip, tolv, res_out);
+    // the tensorial path runs the host-driven fp64 FGMRES: with no fp32 cycles to gain from, its adaptive one-pass
+    // Gram-Schmidt is ~10 % faster than always-CGS2 device cycles (angled_64: 2 109 vs 2 322 ms)
+    if (tensor_) return fgmres(rhs, xsol, iters_out, skip, tolv, res_out);
     auto tol_of = [&](int b) { return tolv ? (*tolv)[b] : opt_.inner_tol; };
     bool ir = kMixed && !tensor_ && !masked_ && opt_.inner_ir != 0;  // the fp32 twin of the operator keeps the PEC model: no masking
     std::vector<char> done(B, 0);
@@ -1851,19 +1813,6 @@ class BatchSolver {
     scale_inv_norm(rhs_, Vout_, hbuf_, hstride());
   }
 
-  // Start vector = normalised sum of the k Ritz vectors of another batch of the same shape (device, [k][Bw][len]): the
-  // Krylov space starts inside the wanted invariant subspace of a neighbouring frequency instead of at a random vector.
-  void init_start_from(const T *warm, int Bw) {
-    std::vector<T> ones((size_t)B * k, from_real<T>(1.0));
-    CUDA_CHECK(cudaMemcpyAsync(qbuf_, ones.data(), ones.size() * sizeof(T), cudaMemcpyHostToDevice, st_));
-    // a shorter last window (Bw > B): problem b starts from problem b of the previous window
-    lincomb(warm, (size_t)Bw * len, qbuf_, k, 1, 1, rhs_, vstride);
-    if (!tensor_) mask_E(rhs_, len);
-    dots(rhs_, 1, rhs_, hbuf_, hstride(), 0, false);
-    scale_inv_norm(rhs_, Vout_, hbuf_, hstride());
-    CUDA_CHECK(cudaStreamSynchronize(st_));
-  }
-
   EigResult krylov_schur(bool real_arith) {
     EigResult out;
     out.theta.assign((size_t)B * k, cd(0, 0));
@@ -1886,7 +1835,7 @@ class BatchSolver {
         double worst = solve_op(vj, w, its, &done, &tolv);
         stats.op_applies++;
         if (!(worst <= 1e-3)) stats.inner_failures++;
-        if (opt_.inner_mode != 0 && j + 2 < kGsMaxCoef) orthonormalise_dev(Vout_, j + 1, w, w, h, nrm, &done);
+        if (j + 2 < kGsMaxCoef) orthonormalise_dev(Vout_, j + 1, w, w, h, nrm, &done);
         else orthonormalise(Vout_, j + 1, w, w, h, nrm);
         for (int b = 0; b < B; ++b) {
           if (done[b]) continue;
